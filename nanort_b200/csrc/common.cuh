@@ -72,6 +72,7 @@ static_assert(sizeof(TraceOptions16) == 16, "BVHTraceOptions layout");
 //   q2 = c1.lo.z, c1.hi.xyz     q3 = ref0, ref1, axis, unused
 // ref >= 0: index of the child's WideNode; ref < 0: leaf, ~ref = first slot in
 // the packed triangle array.  A leaf with no triangles is ref == kEmptyLeaf.
+// The array holds the branch nodes in the nanort array's (depth-first) order, so the root is wide[0].
 struct WideNode {
   float4 q0, q1, q2;
   int4 q3;
@@ -114,7 +115,6 @@ struct Accel {
   uint32_t n_prims = 0;
   size_t n_nodes = 0;
   size_t n_wide = 0;
-  size_t n_top = 0;  // leading WideNodes that form the BFS-ordered top treelet (stageable in shared memory)
   bool root_is_leaf = false;
   // device: reference-layout tree + original geometry (conformance walk)
   Node40 *d_nodes = nullptr;

@@ -94,50 +94,6 @@ __global__ void wide_nodes_kernel(const Node40 *__restrict__ nodes, uint32_t n, 
   wide[widx[i]] = w;
 }
 
-// ---- top treelet: the first kTopNodes WideNodes in breadth-first order go to the front of the array, so that
-// the traversal kernel can stage them into shared memory with a single contiguous TMA bulk copy and address
-// them with the same index (ref < n_top -> shared memory copy).  The rest keeps its depth-first order.
-constexpr uint32_t kTopNodes = 256;
-
-__global__ void bfs_top_kernel(const WideNode *__restrict__ wide, uint32_t n_wide, uint32_t *__restrict__ new_idx,
-                               uint32_t *__restrict__ not_top, uint32_t *n_top_out) {
-  __shared__ uint32_t queue[kTopNodes];
-  if (threadIdx.x != 0) return;
-  uint32_t head = 0, tail = 1;
-  queue[0] = 0;
-  while (head < tail) {
-    const uint32_t i = queue[head];
-    new_idx[i] = head;
-    not_top[i] = 0u;
-    head++;
-    const int4 q3 = wide[i].q3;
-    if (q3.x >= 0 && tail < kTopNodes && (uint32_t)q3.x < n_wide) queue[tail++] = (uint32_t)q3.x;
-    if (q3.y >= 0 && tail < kTopNodes && (uint32_t)q3.y < n_wide) queue[tail++] = (uint32_t)q3.y;
-  }
-  *n_top_out = tail;
-}
-
-__global__ void fill_u32_kernel(uint32_t *p, uint32_t n, uint32_t v) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) p[i] = v;
-}
-
-__global__ void finish_new_idx_kernel(const uint32_t *__restrict__ not_top, const uint32_t *__restrict__ rank,
-                                      const uint32_t *n_top, uint32_t n, uint32_t *__restrict__ new_idx) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n && not_top[i]) new_idx[i] = *n_top + rank[i];
-}
-
-__global__ void remap_wide_kernel(const WideNode *__restrict__ in, const uint32_t *__restrict__ new_idx, uint32_t n,
-                                  WideNode *__restrict__ out) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  WideNode w = in[i];
-  if (w.q3.x >= 0) w.q3.x = (int)new_idx[w.q3.x];
-  if (w.q3.y >= 0) w.q3.y = (int)new_idx[w.q3.y];
-  out[new_idx[i]] = w;
-}
-
 // ---- round-2 layout: PairNode (sign-addressed planes) and TriCM (component-major triangles), derived from the
 // final WideNode / PackedTri arrays so that indices, refs and slots are shared by every kernel
 __global__ void pair_from_wide_kernel(const WideNode *__restrict__ wide, uint32_t n, PairNode *__restrict__ out) {
@@ -170,47 +126,6 @@ __global__ void tris_cm_kernel(const PackedTri *__restrict__ in, uint32_t n, Tri
   o.Y = make_float4(t.a.y, t.b.y, t.c.y, wf);
   o.Z = make_float4(t.a.z, t.b.z, t.c.z, wf);
   out[i] = o;
-}
-
-static int reorder_top_treelet(Accel *a, cudaStream_t s) {
-  const uint32_t n = (uint32_t)a->n_wide;
-  uint32_t *d_new = nullptr, *d_not = nullptr, *d_rank = nullptr, *d_ntop = nullptr;
-  WideNode *d_out = nullptr;
-  cudaError_t ea = cudaMalloc(&d_new, sizeof(uint32_t) * (size_t)n);
-  if (ea == cudaSuccess) ea = cudaMalloc(&d_not, sizeof(uint32_t) * (size_t)n);
-  if (ea == cudaSuccess) ea = cudaMalloc(&d_rank, sizeof(uint32_t) * (size_t)n);
-  if (ea == cudaSuccess) ea = cudaMalloc(&d_ntop, sizeof(uint32_t));
-  if (ea == cudaSuccess) ea = cudaMalloc(&d_out, sizeof(WideNode) * (size_t)n);
-  if (ea == cudaSuccess) {
-    fill_u32_kernel<<<(n + 255) / 256, 256, 0, s>>>(d_not, n, 1u);
-    bfs_top_kernel<<<1, 32, 0, s>>>(a->d_wide, n, d_new, d_not, d_ntop);
-    ea = cudaGetLastError();
-  }
-  uint32_t n_rest = 0;
-  int rc = ea == cudaSuccess ? exclusive_scan_u32(d_not, d_rank, n, &n_rest, s)
-                             : cuda_fail(ea, "reorder_top_treelet", __FILE__, __LINE__);
-  if (rc == NRT_OK) {
-    finish_new_idx_kernel<<<(n + 255) / 256, 256, 0, s>>>(d_not, d_rank, d_ntop, n, d_new);
-    remap_wide_kernel<<<(n + 255) / 256, 256, 0, s>>>(a->d_wide, d_new, n, d_out);
-    uint32_t h_ntop = 0;
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&h_ntop, d_ntop, sizeof(uint32_t), cudaMemcpyDeviceToHost, s);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess) {
-      rc = cuda_fail(e, "reorder_top_treelet", __FILE__, __LINE__);
-    } else {
-      cudaFree(a->d_wide);
-      a->d_wide = d_out;
-      d_out = nullptr;
-      a->n_top = h_ntop;
-    }
-  }
-  cudaFree(d_new);
-  cudaFree(d_not);
-  cudaFree(d_rank);
-  cudaFree(d_ntop);
-  cudaFree(d_out);
-  return rc;
 }
 
 int derive_private_layout(Accel *a, cudaStream_t s) {
@@ -254,8 +169,6 @@ int derive_private_layout(Accel *a, cudaStream_t s) {
   cudaFree(d_flags);  // every path, error or not
   cudaFree(d_widx);
   if (e != cudaSuccess) return cuda_fail(e, "derive_private_layout", __FILE__, __LINE__);
-  if (rc != NRT_OK) return rc;
-  rc = reorder_top_treelet(a, s);
   if (rc != NRT_OK || a->d_prim_boxes) return rc;  // box accels (top level of a scene) are walked by scene.cu only
   NRT_CUDA(cudaMalloc(&a->d_pair, sizeof(PairNode) * a->n_wide));
   NRT_CUDA(cudaMalloc(&a->d_tris_cm, sizeof(TriCM) * (size_t)n_prims));

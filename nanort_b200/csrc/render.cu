@@ -132,9 +132,6 @@ __global__ void __launch_bounds__(256)
 int launch_traverse_soa_devcount(const Accel *a, const float4 *d_org_tmin, const float4 *d_dir_tmax,
                                  const unsigned long long *d_count, size_t capacity, Hit16 *d_hits,
                                  const TraceOptions16 &opt, uint32_t flags, cudaStream_t s);
-int launch_traverse_primary_fused(const Accel *a, const Wave &w, const nrt_ao_params &p, unsigned long long slot0,
-                                  size_t count, float *d_accum, unsigned long long *d_wave_counters,
-                                  const TraceOptions16 &opt, uint32_t flags, cudaStream_t s);
 int launch_traverse_camera_fused(const Accel *a, const Wave &w, const nrt_ao_params &p, unsigned long long slot0,
                                  size_t count, float *d_accum, unsigned long long *d_wave_counters,
                                  const TraceOptions16 &opt, uint32_t flags, cudaStream_t s);

@@ -15,7 +15,7 @@
 // nearest instance boxes in a max-heap that follows libstdc++'s push_heap / pop_heap sift rules, visit them nearest
 // first, walk each instance's nanort-layout tree in the reference's order.  scene_unified_kernel is the production
 // path: persistent warps, one pass over the top-level tree (sub-trees that start behind the current nearest hit are
-// skipped), each candidate instance traversed with the 64-byte child-pair nodes exactly like traverse_fast2_kernel.
+// skipped), each candidate instance traversed with the 64-byte child-pair WideNodes (common.cuh).
 // Both compute the local ray, the world hit point and the world distance with the reference's operation order, so a
 // hit record is bit-identical to the reference's whenever both pick the same (instance, triangle); the pick itself
 // can differ only between candidates at exactly the same world distance.  A ray that pierces more than 64 instance
@@ -405,6 +405,8 @@ constexpr int kSceneBlock = 128;
 //                   unclamped entry distance is not behind the nearest hit (every instance box below starts later)
 //   instance step:  pass iff the slab test over [0, best.t] passes; stack entries are culled against best.t
 constexpr int kUnifiedMinBlocks = 8;  // 64 registers
+constexpr int kUnifiedRefillMin = 16;  // lanes that must have retired before the warp fetches new rays
+constexpr int kUnifiedNodeExit = 8;    // leave the node phase when fewer lanes than this descend
 constexpr int kSentinel = (int)0x80000001;  // ~kSentinel = 0x7FFFFFFE is never a slot
 
 __device__ __forceinline__ bool is_leaf_ref(int r) { return r < 0 && r != kNoLeaf && r != kSentinel; }
@@ -427,7 +429,7 @@ __device__ __forceinline__ bool slab_e(const RayCtx &c, float lox, float loy, fl
   return tmin <= tmax;
 }
 
-template <int LOCAL_DEPTH, int MINB, int REFILL = 16, int NODE_EXIT = 8>
+template <int LOCAL_DEPTH, int MINB>
 __global__ void __launch_bounds__(kSceneBlock, MINB)
     scene_unified_kernel(SceneDev sc, const Ray36 *__restrict__ rays, size_t n, SceneHit32 *__restrict__ hits,
                          uint8_t *__restrict__ mask, uint32_t flags, unsigned long long *cursor,
@@ -490,7 +492,7 @@ __global__ void __launch_bounds__(kSceneBlock, MINB)
   for (;;) {
     // ---- replace retired rays
     const unsigned dead = __ballot_sync(FULL_MASK, ray_idx < 0);
-    if (dead != 0u && !exhausted && (dead == FULL_MASK || __popc(dead) >= REFILL)) {
+    if (dead != 0u && !exhausted && (dead == FULL_MASK || __popc(dead) >= kUnifiedRefillMin)) {
       const int cnt = __popc(dead);
       const int leader = __ffs(dead) - 1;
       unsigned long long base = 0;
@@ -533,7 +535,7 @@ __global__ void __launch_bounds__(kSceneBlock, MINB)
     for (;;) {
       const unsigned desc = __ballot_sync(FULL_MASK, cur >= 0);
       if (desc == 0u) break;
-      if (__popc(desc) < NODE_EXIT && __any_sync(FULL_MASK, leaf != kNoLeaf || cur == kSentinel)) break;
+      if (__popc(desc) < kUnifiedNodeExit && __any_sync(FULL_MASK, leaf != kNoLeaf || cur == kSentinel)) break;
       if (cur >= 0) {
         const float4 *p = reinterpret_cast<const float4 *>(wide + cur);
         const float4 q0 = __ldg(p), q1 = __ldg(p + 1), q2 = __ldg(p + 2);
@@ -707,11 +709,6 @@ static void scene_destroy(Scene *s) {
   delete s;
 }
 
-template <int A, int... R>
-struct FirstArg {
-  static constexpr int value = A;
-};
-
 static int scene_launch(Scene *sc, const Ray36 *d_rays, size_t n, SceneHit32 *d_hits, uint8_t *d_mask, uint32_t flags,
                         cudaStream_t s) {
   if (n == 0) return NRT_OK;
@@ -720,7 +717,6 @@ static int scene_launch(Scene *sc, const Ray36 *d_rays, size_t n, SceneHit32 *d_
     return NRT_ERR_INVALID;
   }
   const SceneDev dev{sc->top->d_nodes, sc->top->d_indices, sc->d_inst, sc->top->d_wide, sc->top->d_tris};
-  const uint32_t variant = (flags >> 8) & 0xFFu;  // policy variants for A/B runs (tools/scene_sweep.py); 0 = default
   const uint32_t stack_need = sc->top->stats.max_tree_depth + sc->max_blas_depth + 6;
   const bool list_only = (flags & NRT_TRAVERSE_CONFORMANCE) != 0 || stack_need > 1024;
   const int sms = device_sm_count(sc->device);
@@ -729,6 +725,10 @@ static int scene_launch(Scene *sc, const Ray36 *d_rays, size_t n, SceneHit32 *d_
     scene_list_kernel<<<(unsigned)blocks, 128, 0, s>>>(dev, d_rays, n, nullptr, nullptr, d_hits, d_mask, flags);
     NRT_CUDA(cudaGetLastError());
     return NRT_OK;
+  }
+  if (stack_need <= 64 && ((flags >> 8) & 0xFFu) != 0) {  // the list-only and deep-stack walks ignore them
+    set_error("nrt_scene_traverse: flags bits 8..15 are reserved");
+    return NRT_ERR_INVALID;
   }
   const int slot = (int)(sc->ring.fetch_add(1) % (uint32_t)Scene::kSlots);
   uint32_t *d_overflow = nullptr;
@@ -748,42 +748,18 @@ static int scene_launch(Scene *sc, const Ray36 *d_rays, size_t n, SceneHit32 *d_
   NRT_CUDA(cudaMemsetAsync(cursor, 0, sizeof(unsigned long long), s));
   NRT_CUDA(cudaMemsetAsync(ovf, 0, sizeof(unsigned long long), s));
   const size_t need = ((n + 31) / 32 + 3) / 4;
-  {
-    size_t grid = (size_t)sms * (stack_need > 64 ? 2 : kUnifiedMinBlocks);
-    if (grid > need) grid = need;
-    if (stack_need > 64)
-      scene_unified_kernel<1024, 2><<<(unsigned)grid, kSceneBlock, 0, s>>>(dev, d_rays, n, d_hits, d_mask, flags, cursor,
-                                                                        d_overflow, ovf);
-    else if (variant != 0) {
-#define NRT_SCENE_VARIANT(id, ...)                                                                              \
-  case id: {                                                                                                    \
-    size_t g = std::min(need, (size_t)sms * (FirstArg<__VA_ARGS__>::value));                                    \
-    scene_unified_kernel<64, __VA_ARGS__><<<(unsigned)g, kSceneBlock, 0, s>>>(dev, d_rays, n, d_hits, d_mask,   \
-                                                                              flags, cursor, d_overflow, ovf); \
-  } break;
-      switch (variant) {
-        NRT_SCENE_VARIANT(2, 6, 16, 8)
-        NRT_SCENE_VARIANT(3, 8, 16, 8)
-        NRT_SCENE_VARIANT(4, 5, 16, 8)
-        NRT_SCENE_VARIANT(5, 7, 8, 8)
-        NRT_SCENE_VARIANT(6, 7, 24, 8)
-        NRT_SCENE_VARIANT(7, 7, 16, 4)
-        NRT_SCENE_VARIANT(8, 7, 16, 12)
-        NRT_SCENE_VARIANT(9, 7, 16, 16)
-        default:
-          set_error("nrt_scene_traverse: unknown kernel variant in flags");
-          return NRT_ERR_INVALID;
-      }
-#undef NRT_SCENE_VARIANT
-    } else
-      scene_unified_kernel<64, kUnifiedMinBlocks><<<(unsigned)grid, kSceneBlock, 0, s>>>(
-          dev, d_rays, n, d_hits, d_mask, flags, cursor, d_overflow, ovf);
-    NRT_CUDA(cudaGetLastError());
-    scene_list_kernel<<<(unsigned)std::min<size_t>((n + 127) / 128, (size_t)sms * 4), 128, 0, s>>>(
-        dev, d_rays, n, d_overflow, ovf, d_hits, d_mask, flags);
-    NRT_CUDA(cudaGetLastError());
-    return NRT_OK;
-  }
+  size_t grid = (size_t)sms * (stack_need > 64 ? 2 : kUnifiedMinBlocks);
+  if (grid > need) grid = need;
+  if (stack_need > 64)
+    scene_unified_kernel<1024, 2><<<(unsigned)grid, kSceneBlock, 0, s>>>(dev, d_rays, n, d_hits, d_mask, flags, cursor,
+                                                                      d_overflow, ovf);
+  else
+    scene_unified_kernel<64, kUnifiedMinBlocks><<<(unsigned)grid, kSceneBlock, 0, s>>>(
+        dev, d_rays, n, d_hits, d_mask, flags, cursor, d_overflow, ovf);
+  NRT_CUDA(cudaGetLastError());
+  scene_list_kernel<<<(unsigned)std::min<size_t>((n + 127) / 128, (size_t)sms * 4), 128, 0, s>>>(
+      dev, d_rays, n, d_overflow, ovf, d_hits, d_mask, flags);
+  NRT_CUDA(cudaGetLastError());
   return NRT_OK;
 }
 

@@ -1,6 +1,13 @@
-// Round-2 production traversal kernel (sm_90a).  Same algorithm and the same arithmetic as traverse_fast2_kernel
-// (persistent warps, ray pool refilled by warp ballot, while-while with one postponed leaf per lane, per-lane stack
-// of (ref, entry distance)), re-shaped by what the round-1 profiles showed:
+// Production traversal kernel (sm_90a).  Persistent warps pull rays from a global cursor and replace finished rays
+// with new ones once enough lanes of the warp have retired (warp-ballot compaction of the ray pool).  Traversal is
+// while-while with one postponed leaf per lane over child-pair nodes; the per-lane stack keeps (ref, entry distance)
+// so that a popped subtree that now lies behind the current best is skipped without touching memory -- the same visit
+// set the reference obtains by re-testing the box when it is popped (nanort.h:2532).
+//
+// Its first version was issue bound, with ~29 % of the issued instructions being control flow, hence: a triangle test
+// without early returns (one predicate at the end; only the fp64 fallback branches), empty children that carry an
+// inverted box (no reference checks in the node step), child selection by selects and one predicated push.  The
+// profiles of that version further showed:
 //
 //   * 12 of the 54 instructions of a child-pair slab test were FSELs picking bmin/bmax by ray_dir_sign
 //     (nanort.h:2291-2302) and they sit on the half-rate ALU pipe (60 % busy)  -> PairNode: the selection is an
@@ -128,22 +135,21 @@ __device__ __forceinline__ void tri_test3(const RayCtx3 &c, const TraceOptions16
 
 constexpr int kNone3 = kEmptyLeaf;  // "no node": finished, or (with a non-empty stack) waiting for a pop
 
-template <int BLOCK_, int MINB_, int REFILL_MIN_, int NODE_EXIT_, bool PAIR128_ = true, int LEAF_AGAIN_MIN_ = 1,
-          int LEAF_SLOTS_ = 1, bool DEFER_RETIRE_ = false, int NODE_UNROLL_ = 1>
+constexpr int kTraverseBlock = 128;  // threads per CTA
+constexpr int kNodeExit = 8;         // leave the node phase when fewer lanes than this want node work
+
+// Launch policy of traverse_fast3_kernel (the values and why: traverse.cu)
+template <int MINB_, int REFILL_MIN_, bool PAIR128_, int LEAF_AGAIN_MIN_, bool DEFER_RETIRE_, int NODE_UNROLL_>
 struct Policy3 {
-  static constexpr int kBlock = BLOCK_;
-  static constexpr int kMinBlocks = MINB_;
+  static constexpr int kMinBlocks = MINB_;        // CTAs per SM (the register budget) and of the persistent grid
   static constexpr int kRefillMin = REFILL_MIN_;  // lanes that must have retired before the warp fetches new rays
-  static constexpr int kNodeExit = NODE_EXIT_;    // leave the node phase when fewer lanes than this want node work
   // true: 128-byte PairNode (sign-addressed planes, no selects); false: the 64-byte WideNode with 12 selects per pair
-  // (half the cache footprint per node) -- A/B knob (kernel variants of nrt_traverse)
+  // (half the cache footprint per node)
   static constexpr bool kPair128 = PAIR128_;
   // after the first leaf round of an outer iteration, another one runs only while at least this many lanes hold a
   // leaf (1: until none is left; 33: one round) -- a lane's second leaf (found while the first was postponed) is
   // otherwise tested in a round of its own with the few lanes that have one; carried over, it joins the next phase's
   static constexpr int kLeafAgainMin = LEAF_AGAIN_MIN_;
-  // postponed leaves a lane may hold before it parks (1 or 2)
-  static constexpr int kLeafSlots = LEAF_SLOTS_;
   // true: finished rays wait for the retire step until retired + empty lanes reach kRefillMin (or nothing else is
   // left to do), so that the epilogue and the refill that follows run with more lanes
   static constexpr bool kDeferRetire = DEFER_RETIRE_;
@@ -154,7 +160,7 @@ struct Policy3 {
 // DEPTH: capacity of the per-lane stack (entries); chosen by the launcher from the tree depth, so a push can
 // never overflow (a child pair pushes one entry and descends one level).
 template <class Rays, int DEPTH, bool COUNT, class P, class Epi>
-__global__ void __launch_bounds__(P::kBlock, P::kMinBlocks)
+__global__ void __launch_bounds__(kTraverseBlock, P::kMinBlocks)
     traverse_fast3_kernel(const void *__restrict__ pair, const TriCM *__restrict__ tris, Rays rays, size_t n, Epi epi,
                           TraceOptions16 opt, uint32_t flags, unsigned long long *cursor, unsigned long long *counts,
                           const unsigned long long *n_ptr) {
@@ -177,7 +183,6 @@ __global__ void __launch_bounds__(P::kBlock, P::kMinBlocks)
   float min_t = 0.0f;
   bool alive = false;
   int cur = kNone3, leaf = kNone3;
-  int leaf2 = kNone3;  // second postponed leaf (P::kLeafSlots == 2 only; leaf2 != kNone3 implies leaf != kNone3)
   bool exhausted = false;
   unsigned long long n_boxes = 0, n_prims = 0;
   // COUNT only: lane-state histogram of the warp's iterations (nrt_traverse_lane_stats_device; lane 0 accumulates)
@@ -217,7 +222,6 @@ __global__ void __launch_bounds__(P::kBlock, P::kMinBlocks)
           sp = 0;
           cur = range_has_nan(min_t, max_t) ? kNone3 : 0;
           leaf = kNone3;
-          leaf2 = kNone3;
           if (COUNT) n_boxes += 1;
         }
       }
@@ -232,7 +236,7 @@ __global__ void __launch_bounds__(P::kBlock, P::kMinBlocks)
       bool want = cur >= 0 || (cur == kNone3 && sp > 0);
       const unsigned desc = __ballot_sync(FULL_MASK, want);
       if (desc == 0u) break;
-      if (P::kNodeExit > 1 && __popc(desc) < P::kNodeExit && __any_sync(FULL_MASK, leaf != kNone3)) break;
+      if (__popc(desc) < kNodeExit && __any_sync(FULL_MASK, leaf != kNone3)) break;
 #pragma unroll
       for (int rep = 0; rep < P::kNodeUnroll; ++rep) {
         if (rep > 0) want = cur >= 0 || (cur == kNone3 && sp > 0);
@@ -248,9 +252,6 @@ __global__ void __launch_bounds__(P::kBlock, P::kMinBlocks)
               cur = (int)e.x;
               if (cur < 0 && leaf == kNone3) {
                 leaf = cur;
-                cur = kNone3;
-              } else if (P::kLeafSlots == 2 && cur < 0 && leaf2 == kNone3) {
-                leaf2 = cur;
                 cur = kNone3;
               }
             }
@@ -293,9 +294,6 @@ __global__ void __launch_bounds__(P::kBlock, P::kMinBlocks)
             if (cur < 0 && cur != kNone3 && leaf == kNone3) {  // postpone the first leaf, keep descending
               leaf = cur;
               cur = kNone3;
-            } else if (P::kLeafSlots == 2 && cur < 0 && cur != kNone3 && leaf2 == kNone3) {
-              leaf2 = cur;
-              cur = kNone3;
             }
           }
         }
@@ -325,18 +323,9 @@ __global__ void __launch_bounds__(P::kBlock, P::kMinBlocks)
           slot++;
         }
         leaf = kNone3;
-        if (P::kLeafSlots == 2) {
-          leaf = leaf2;
-          leaf2 = kNone3;
-        }
         if (cur < 0 && cur != kNone3) {  // a leaf was waiting in cur (the lane was parked)
-          if (leaf == kNone3) {
-            leaf = cur;
-            cur = kNone3;
-          } else if (P::kLeafSlots == 2) {  // leaf2 was just vacated
-            leaf2 = cur;
-            cur = kNone3;
-          }
+          leaf = cur;
+          cur = kNone3;
         }
         // occlusion query (NRT_TRAVERSE_ANY_HIT): a hit inside [min_t, max_t) ends the ray.  A record accepted AT
         // max_t is a miss (nanort.h:2552) and does not.
@@ -344,7 +333,6 @@ __global__ void __launch_bounds__(P::kBlock, P::kMinBlocks)
           sp = 0;
           cur = kNone3;
           leaf = kNone3;
-          leaf2 = kNone3;
         }
       }
     }

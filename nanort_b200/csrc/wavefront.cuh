@@ -237,7 +237,7 @@ __device__ __forceinline__ void make_ao_ray(const nrt_ao_params &p, uint32_t pix
   d4 = make_float4(wx * il, wy * il, wz * il, p.ao_max_t);
 }
 
-// ---- retire-step functors of traverse_fast2_kernel.  Called by ALL 32 lanes of a warp (`retiring` says
+// ---- retire-step functors of traverse_fast3_kernel.  Called by ALL 32 lanes of a warp (`retiring` says
 // whether this lane's ray just finished), so they may use full-mask warp votes.
 struct StoreHitsEpilogue {
   static constexpr bool kAnyHit = false;  // true: the kernel retires a ray at its first hit inside [min_t, max_t)
@@ -254,13 +254,11 @@ struct StoreHitsEpilogue {
   }
 };
 
-// primary rays: a hit spawns its AO ray straight into the compacted AO queue, a miss adds 1 to its pixel.
-// GEN: the primary rays were generated in the kernel (CameraRays) -- pixel and ray are recomputed from the slot.
-template <bool GEN>
+// camera rays generated in the kernel (CameraRays): a hit spawns its AO ray straight into the compacted AO queue, a
+// miss adds 1 to its pixel.  Pixel and ray come back from the payload the ray loader parked.
 struct PrimaryToAoEpilogue {
   static constexpr bool kAnyHit = false;
   nrt_ao_params p;
-  unsigned long long slot0;
   Wave w;
   const float *verts;
   const uint32_t *faces;
@@ -274,27 +272,13 @@ struct PrimaryToAoEpilogue {
     float4 o4 = make_float4(0.f, 0.f, 0.f, 0.f), d4 = o4;
     uint32_t pix = 0xFFFFFFFFu, acc = 0;
     if (retiring) {
-      uint32_t smp = 0;
-      float4 ro, rd;
-      if (GEN) {  // the camera ray's payload (CameraRays::load): direction, pixel, sample, accumulation index
-        pix = payload[3];
-        if (pix != 0xFFFFFFFFu) {
-          smp = payload[4];
-          acc = payload[5];
-          ro = make_float4(p.cam[0], p.cam[1], p.cam[2], p.ray_min_t);
-          rd = make_float4(__uint_as_float(payload[0]), __uint_as_float(payload[1]), __uint_as_float(payload[2]),
-                           p.ray_max_t);
-        }
-      } else {
-        pix = w.pix[ray_idx];
-        acc = pix;  // the unfused path does not pack (run_ao_pass rejects the combination)
-        if (pix != 0xFFFFFFFFu) {
-          smp = slot_sample(p, slot0 + ray_idx);
-          ro = w.org_tmin[ray_idx];
-          rd = w.dir_tmax[ray_idx];
-        }
-      }
+      pix = payload[3];  // the camera ray's payload (CameraRays::load): direction, pixel, sample, accumulation index
       if (pix != 0xFFFFFFFFu) {
+        const uint32_t smp = payload[4];
+        acc = payload[5];
+        const float4 ro = make_float4(p.cam[0], p.cam[1], p.cam[2], p.ray_min_t);
+        const float4 rd = make_float4(__uint_as_float(payload[0]), __uint_as_float(payload[1]),
+                                      __uint_as_float(payload[2]), p.ray_max_t);
         if (t < max_t) {
           make_ao_ray(p, pix, smp, ro, rd, t, prim, verts, faces, o4, d4);
           make = true;

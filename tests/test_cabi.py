@@ -74,7 +74,7 @@ def test_python_mirror_constants_equal_the_header_defines():
     for name, value in pairs.items():
         assert name in defs, name
         assert defs[name] == value, (name, defs[name], value)
-    # the traverse flag bits do not collide with each other or with the experiment selector (bits 8..15)
+    # the traverse flag bits do not collide with each other or with the reserved bits 8..15
     bits = [defs[n] for n in ("NRT_TRAVERSE_CONFORMANCE", "NRT_TRAVERSE_CPP03_INVERSE", "NRT_TRAVERSE_RAY32", "NRT_TRAVERSE_ANY_HIT")]
     assert len(set(bits)) == 4 and all(b & (b - 1) == 0 and b < 0x100 for b in bits)
     assert defs["NRT_AO_UNFUSED"] > 0xFFFF and defs["NRT_AO_PACKED_TILES"] > 0xFFFF

@@ -77,7 +77,20 @@ def test_traverse_and_render_reject_null_and_bad_tiles():
     p.tile_w, p.shard, p.n_shards = 64, 3, 2  # shard outside the shard count
     with pytest.raises(api.NanortB200Error):
         acc.RenderAO(p, accum.data_ptr())
-    # an unknown kernel-variant selector in the flags is refused, not ignored
+    # a non-zero value in the reserved flags bits 8..15 is refused, not ignored
     rays = np.zeros(4, np.dtype([("o", "<f4", 3), ("d", "<f4", 3), ("a", "<f4"), ("b", "<f4"), ("t", "<u4")]))
+    for sel in (1, 100, 200):
+        with pytest.raises(api.NanortB200Error):
+            acc.Traverse(rays, flags=(sel << 8))
+    # the same for the two-level scene's production walk (a shallow scene: the deep-stack and list-only walks
+    # ignore those bits)
+    sc = api.Scene()
+    sc.AddNode(acc, np.eye(4, dtype=np.float32))
+    assert sc.Commit()
+    rays["o"] = (0.2, 0.2, -1.0)
+    rays["d"] = (0.0, 0.0, 1.0)
+    rays["b"] = 1e30
+    h, m = sc.Traverse(rays)
+    assert m.all()
     with pytest.raises(api.NanortB200Error):
-        acc.Traverse(rays, flags=(200 << 8))
+        sc.Traverse(rays, flags=(2 << 8))

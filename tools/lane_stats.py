@@ -25,16 +25,15 @@ for scene in scenes:
     d_a = torch.empty(n * 36, dtype=torch.uint8, device="cuda")
     n_p, n_a = acc.ExportAOWorkload(p, accum.data_ptr(), d_p.data_ptr(), d_a.data_ptr())
     for name, d_r, cnt in (("primary", d_p, n_p), ("ao", d_a, n_a)):
-        for var in [int(x) for x in (sys.argv[2].split(",") if len(sys.argv) > 2 else ["0"])]:
-            s = acc.LaneStatsDevice(d_r.data_ptr(), cnt, flags=(var << 8))
-            ns, lr, ts = max(s["node_steps"], 1), max(s["leaf_rounds"], 1), max(s["tri_steps"], 1)
-            print(json.dumps({"scene": scene, "rays": name, "variant": var, "n": cnt,
-                              "node_steps_per_ray": s["boxes"] / 2 / cnt, "prims_per_ray": s["prims"] / cnt,
-                              "node_phase_lanes": {"testing": s["lanes_testing"] / ns, "no_ray": s["lanes_no_ray"] / ns,
-                                                   "finished": s["lanes_finished"] / ns,
-                                                   "parked_on_leaves": s["lanes_parked_on_leaves"] / ns},
-                              "leaf_round_lanes": s["lanes_with_leaf"] / lr, "tri_step_lanes": s["prims"] / ts,
-                              "tri_steps_per_round": ts / lr, "node_steps_per_outer": ns / max(s["outer_iterations"], 1),
-                              "refill_lanes": s["lanes_refilled"] / max(s["refill_events"], 1),
-                              "retire_lanes": s["lanes_retired"] / max(s["retire_events"], 1),
-                              "outer_per_ray_x32": 32 * s["outer_iterations"] / cnt, "raw": s}), flush=True)
+        s = acc.LaneStatsDevice(d_r.data_ptr(), cnt)
+        ns, lr, ts = max(s["node_steps"], 1), max(s["leaf_rounds"], 1), max(s["tri_steps"], 1)
+        print(json.dumps({"scene": scene, "rays": name, "n": cnt,
+                          "node_steps_per_ray": s["boxes"] / 2 / cnt, "prims_per_ray": s["prims"] / cnt,
+                          "node_phase_lanes": {"testing": s["lanes_testing"] / ns, "no_ray": s["lanes_no_ray"] / ns,
+                                               "finished": s["lanes_finished"] / ns,
+                                               "parked_on_leaves": s["lanes_parked_on_leaves"] / ns},
+                          "leaf_round_lanes": s["lanes_with_leaf"] / lr, "tri_step_lanes": s["prims"] / ts,
+                          "tri_steps_per_round": ts / lr, "node_steps_per_outer": ns / max(s["outer_iterations"], 1),
+                          "refill_lanes": s["lanes_refilled"] / max(s["refill_events"], 1),
+                          "retire_lanes": s["lanes_retired"] / max(s["retire_events"], 1),
+                          "outer_per_ray_x32": 32 * s["outer_iterations"] / cnt, "raw": s}), flush=True)

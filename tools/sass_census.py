@@ -1,6 +1,6 @@
 """Opcode census of the built library (cuobjdump -sass): which kernels use FFMA/DFMA (only inside IEEE division
-sequences under --fmad=false), REDUX/MATCH (warp-aggregated binning), UBLKCP/SYNCS (TMA bulk copy + mbarrier).
-usage: python tools/sass_census.py > profiles/rNN_sass_census.md"""
+sequences under --fmad=false), REDUX/MATCH (warp-aggregated binning).
+usage: python tools/sass_census.py > sass_census.md"""
 import collections, os, re, subprocess
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -16,19 +16,17 @@ for l in sass.splitlines():
     m = re.match(r"\s*/\*[0-9a-f]+\*/\s+(@!?U?P\d\s+)?([A-Z0-9_.]+)", l)
     if cur and m:
         ops[cur].append(m.group(2))
-WANT = ["traverse_fast2_kernelINS_10CameraRaysELi48ELb0ENS_10FastPolicyILi128ELi10ELi16ELi8ELi0ELi0", "AoAccumulateEpilogue",
-        "traverse_conformance_kernelINS_7AosRaysELb0", "FastPolicyILi128ELi10ELi16ELi8ELi64ELi16EEENS_17StoreHits",
-        "scene_unified_kernelILi64ELi8E", "scene_list_kernel", "traverse_f64_kernel", "bin_large_kernel", "subtree_kernel",
+WANT = ["traverse_fast3_kernel", "traverse_conformance_kernelINS_7AosRaysELb0", "scene_unified_kernelILi64ELi8E", "scene_list_kernel", "traverse_f64_kernel", "bin_large_kernel", "subtree_kernel",
         "instance_setup_kernel"]
-print("| kernel | SASS instrs | FFMA/DFMA | ... of them within a division / sqrt sequence | FMUL+FADD (DMUL+DADD) | MUFU | REDUX | MATCH | UBLKCP | SYNCS |")
-print("|---|---|---|---|---|---|---|---|---|---|")
+print("| kernel | SASS instrs | FFMA/DFMA | ... of them within a division / sqrt sequence | FMUL+FADD (DMUL+DADD) | MUFU | REDUX | MATCH |")
+print("|---|---|---|---|---|---|---|---|")
 seen = set()
 for name, lst in ops.items():
     if not any(w in name for w in WANT):
         continue
     dem = subprocess.run(["c++filt", name], capture_output=True, text=True).stdout.strip()
-    dem = re.sub(r"nrt::\(anonymous namespace\)::|nrt::", "", dem).split("(")[0][:90]
-    if dem in seen or "Li496" in name:
+    dem = re.sub(r"nrt::\(anonymous namespace\)::|nrt::", "", dem).split("(")[0][:160]
+    if dem in seen or "Li512" in name:  # the deep-stack twin of a 64-entry instantiation
         continue
     seen.add(dem)
     c = collections.Counter(x.split(".")[0] for x in lst)
@@ -37,4 +35,4 @@ for name, lst in ops.items():
     # the division slow path is a local subroutine whose FFMAs carry explicit rounding modes (.RZ/.RM/.RP)
     inside = sum(1 for i in fma if (anchors and min(abs(i - a) for a in anchors) <= 28) or re.search(r"\.R[ZMP]", lst[i]))
     print(f"| `{dem}` | {len(lst)} | {len(fma)} | {inside} | {c['FMUL'] + c['FADD']} ({c['DMUL'] + c['DADD']}) | {c['MUFU']} | "
-          f"{c['REDUX']} | {c['MATCH']} | {c['UBLKCP']} | {c['SYNCS']} |")
+          f"{c['REDUX']} | {c['MATCH']} |")
