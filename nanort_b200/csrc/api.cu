@@ -176,12 +176,6 @@ bool validate_foreign_tree(const Node40 *hn, size_t n_nodes, const uint32_t *ind
 }
 bool validate_foreign_tree64(const void *nodes_64B, size_t n_nodes, const uint32_t *indices, size_t n_indices,
                              uint32_t n_prims, BuildStats16 *stats, std::string *why) {
-  struct Node64 {
-    double bmin[3], bmax[3];
-    int32_t flag, axis;
-    uint32_t data[2];
-  };
-  static_assert(sizeof(Node64) == 64, "BVHNode<double> layout");
   return validate_foreign_tree_t(static_cast<const Node64 *>(nodes_64B), n_nodes, indices, n_indices, n_prims, stats, why);
 }
 

@@ -8,6 +8,7 @@
 #include <condition_variable>
 #include <mutex>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/nanort_b200.h"
@@ -23,6 +24,18 @@ struct Node40 {
   uint32_t data[2];  // leaf {count, first}; branch {left, right}
 };
 static_assert(sizeof(Node40) == 40, "BVHNode<float> layout");
+
+struct Node64 {  // Node40 with double boxes
+  double bmin[3];
+  double bmax[3];
+  int32_t flag;
+  int32_t axis;
+  uint32_t data[2];
+};
+static_assert(sizeof(Node64) == 64, "BVHNode<double> layout");
+
+template <typename T>
+using BVHNodeOf = typename std::conditional<std::is_same<T, float>::value, Node40, Node64>::type;
 
 struct Ray36 {
   float org[3];
@@ -246,7 +259,17 @@ int launch_traverse_soa(const Accel *a, const float4 *d_org_tmin, const float4 *
 int derive_private_layout(Accel *a, cudaStream_t s);
 // build.cu
 int build_on_device(Accel *a, cudaStream_t s);
-// build_ref.cu
+// build_ref.cu: the reference-exact builder of BVHAccel<T>, T = float or double.  Inputs on the device: packed T
+// vertices + faces, or (T = float only) d_boxes, 6 floats per box primitive.  cpp11_order: emit the node order of the
+// C++11 parallel build when n > min_primitives_for_parallel_build.  On success *d_nodes_out (2n+2 capacity) and
+// *d_indices_out (n) are device arrays the caller owns.
+template <typename T>
+int build_reference_tree(const T *d_verts, const uint32_t *d_faces, const float *d_boxes, uint32_t n,
+                         uint32_t bin_size, uint32_t min_leaf_primitives, uint32_t max_tree_depth,
+                         uint32_t shallow_depth, uint32_t min_primitives_for_parallel_build, bool cpp11_order,
+                         BVHNodeOf<T> **d_nodes_out, uint32_t **d_indices_out, size_t *n_nodes_out,
+                         BuildStats16 *stats_out, T root_bmin[3], T root_bmax[3], cudaStream_t s);
+// the float builder over an accel's geometry (or its box primitives), writing its arrays, statistics and root box
 int build_reference_tree_on_device(Accel *a, bool cpp11_order, cudaStream_t s);
 
 // prims.cu

@@ -26,21 +26,8 @@
 #include "scan.cuh"
 
 namespace nrt {
-
-int build_reference_tree_f64_on_device(const double *d_verts, const uint32_t *d_faces, uint32_t n, uint32_t bin_size,
-                                       uint32_t min_leaf_primitives, uint32_t max_tree_depth, uint32_t shallow_depth,
-                                       uint32_t min_primitives_for_parallel_build, bool cpp11_order, void **d_nodes_out,
-                                       uint32_t **d_indices_out, size_t *n_nodes_out, BuildStats16 *stats_out,
-                                       double root_bmin[3], double root_bmax[3], cudaStream_t s);
-
 namespace {
 
-struct Node64 {
-  double bmin[3], bmax[3];
-  int32_t flag, axis;
-  uint32_t data[2];
-};
-static_assert(sizeof(Node64) == 64, "BVHNode<double> layout");
 struct Ray72 {
   double org[3], dir[3], min_t, max_t;
   uint32_t type, pad;
@@ -495,16 +482,14 @@ int nrt_build_f64_ex(const double *verts, size_t stride_bytes, size_t n_verts, c
     F64_CUDA(cudaStreamSynchronize(a->stream));
   }
   if (flags & NRT_BUILD_REFERENCE_TREE) {
-    // conformance build: the reference's own BVHNode<double> array and indices_, bit for bit (build_ref64.cu)
-    void *d_nodes = nullptr;
+    // conformance build: the reference's own BVHNode<double> array and indices_, bit for bit (build_ref.cu)
     cudaFree(t->d_verts);
     t->d_verts = nullptr;
-    rc = build_reference_tree_f64_on_device(a->d_verts, a->d_faces, n_prims, o64.bin_size, o64.min_leaf_primitives,
-                                            o64.max_tree_depth, o64.shallow_depth, o64.min_primitives_for_parallel_build,
-                                            (flags & NRT_BUILD_REFERENCE_CPP03_ORDER) == 0, &d_nodes, &a->d_indices,
-                                            &a->n_nodes, &a->stats, a->root_bmin, a->root_bmax, a->stream);
+    rc = build_reference_tree<double>(a->d_verts, a->d_faces, nullptr, n_prims, o64.bin_size, o64.min_leaf_primitives,
+                                      o64.max_tree_depth, o64.shallow_depth, o64.min_primitives_for_parallel_build,
+                                      (flags & NRT_BUILD_REFERENCE_CPP03_ORDER) == 0, &a->d_nodes, &a->d_indices,
+                                      &a->n_nodes, &a->stats, a->root_bmin, a->root_bmax, a->stream);
     if (rc != NRT_OK) goto fail;
-    a->d_nodes = static_cast<Node64 *>(d_nodes);
     delete t;
     *out = reinterpret_cast<nrt_accel_f64 *>(a);
     return NRT_OK;
