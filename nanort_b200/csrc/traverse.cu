@@ -103,6 +103,7 @@ __global__ void __launch_bounds__(128)
     float hit_t = max_t;
     uint32_t stack[kConfStack];
     int sp = range_has_nan(min_t, max_t) ? -1 : 0;
+    if (COUNT && sp < 0) n_boxes++;  // the reference still pops the root, whose slab test then fails
     stack[0] = 0;
     while (sp >= 0) {
       const Node40 *nd = nodes + stack[sp];
@@ -133,6 +134,13 @@ __global__ void __launch_bounds__(128)
           if (tri_test(c, opt, a, b, cc, best)) any = true;
         }
         if (any) hit_t = best.t;
+        // A ray with a NaN or infinite origin / direction can accept a triangle at t = NaN (no comparison rejects it).
+        // The reference's safemin then makes every later slab test fail: it pops what is left on the stack and visits
+        // nothing else.  fminf drops the NaN and would walk on; the hit record is a miss either way.
+        if (COUNT && hit_t != hit_t) {
+          n_boxes += (unsigned long long)(sp + 1);
+          break;
+        }
       }
     }
     if (hits) write_result(hits, mask, i, best, max_t);
@@ -368,6 +376,7 @@ int launch_traverse_count(const Accel *a, const Ray36 *d_rays, size_t n, const T
   if (n == 0) return NRT_OK;
   AosRays r{d_rays};
   unsigned long long *cnt = reinterpret_cast<unsigned long long *>(d_counts2);
+  flags = (flags & ~kCountRootIsLeaf) | (a->root_is_leaf ? kCountRootIsLeaf : 0u);
   if (flags & NRT_TRAVERSE_CONFORMANCE) return launch_conf<AosRays, true>(a, r, n, nullptr, nullptr, opt, flags, cnt, s);
   return launch_fast<AosRays, true>(a, r, n, nullptr, nullptr, opt, flags, cnt, s);
 }

@@ -82,15 +82,41 @@ __device__ __forceinline__ void slab_pair(const RayCtx3 &c, const float4 X, cons
   h1 = t1 <= e1;
 }
 
-// Same for the 64-byte WideNode (q0 = c0.lo.xyz, c0.hi.x | q1 = c0.hi.yz, c1.lo.xy | q2 = c1.lo.z, c1.hi.xyz): the
-// planes are picked by the ray's direction signs with selects.
+// The planes of a 64-byte WideNode (q0 = c0.lo.xyz, c0.hi.x | q1 = c0.hi.yz, c1.lo.xy | q2 = c1.lo.z, c1.hi.xyz) in
+// the PairNode order {near0 near1 far0 far1}, picked by the ray's direction signs with selects.
+__device__ __forceinline__ void wide_planes(const RayCtx3 &c, const float4 q0, const float4 q1, const float4 q2, float4 &X,
+                                            float4 &Y, float4 &Z) {
+  const bool sx = (c.nx & 1u) != 0u, sy = (c.ny & 1u) != 0u, sz = (c.nz & 1u) != 0u;
+  X = make_float4(sx ? q0.w : q0.x, sx ? q2.y : q1.z, sx ? q0.x : q0.w, sx ? q1.z : q2.y);
+  Y = make_float4(sy ? q1.x : q0.y, sy ? q2.z : q1.w, sy ? q0.y : q1.x, sy ? q1.w : q2.z);
+  Z = make_float4(sz ? q1.y : q0.z, sz ? q2.w : q2.x, sz ? q0.z : q1.y, sz ? q2.x : q2.w);
+}
+
+// slab_pair on the WideNode
 __device__ __forceinline__ void slab_pair_sel(const RayCtx3 &c, const float4 q0, const float4 q1, const float4 q2,
                                               float min_t, float best_t, bool &h0, bool &h1, float &t0, float &t1) {
-  const bool sx = (c.nx & 1u) != 0u, sy = (c.ny & 1u) != 0u, sz = (c.nz & 1u) != 0u;
-  const float4 X = make_float4(sx ? q0.w : q0.x, sx ? q2.y : q1.z, sx ? q0.x : q0.w, sx ? q1.z : q2.y);
-  const float4 Y = make_float4(sy ? q1.x : q0.y, sy ? q2.z : q1.w, sy ? q0.y : q1.x, sy ? q1.w : q2.z);
-  const float4 Z = make_float4(sz ? q1.y : q0.z, sz ? q2.w : q2.x, sz ? q0.z : q1.y, sz ? q2.x : q2.w);
+  float4 X, Y, Z;
+  wide_planes(c, q0, q1, q2, X, Y, Z);
   slab_pair(c, X, Y, Z, min_t, best_t, h0, h1, t0, t1);
+}
+
+// Slab test of the union of a pair's two child boxes, in the arithmetic of slab() (trav_common.cuh): the union's near
+// plane is the nearer of the two near planes, its far plane the farther of the two far planes.  Every tree our builders
+// or the reference emit has exact-union boxes, so on the root pair this is the reference's test of the root box
+// (nanort.h:2527-2530).  An empty child's inverted box never wins either choice.  Used by the visit counters only.
+__device__ __forceinline__ bool slab_union(const RayCtx3 &c, const float4 X, const float4 Y, const float4 Z, float min_t,
+                                           float max_t) {
+  const bool sx = (c.nx & 1u) != 0u, sy = (c.ny & 1u) != 0u, sz = (c.nz & 1u) != 0u;
+  const float nx = sx ? fmaxf(X.x, X.y) : fminf(X.x, X.y), fx = sx ? fminf(X.z, X.w) : fmaxf(X.z, X.w);
+  const float ny = sy ? fmaxf(Y.x, Y.y) : fminf(Y.x, Y.y), fy = sy ? fminf(Y.z, Y.w) : fmaxf(Y.z, Y.w);
+  const float nz = sz ? fmaxf(Z.x, Z.y) : fminf(Z.x, Z.y), fz = sz ? fminf(Z.z, Z.w) : fmaxf(Z.z, Z.w);
+  const float tnx = (nx - c.ox) * c.ix, tny = (ny - c.oy) * c.iy, tnz = (nz - c.oz) * c.iz;
+  const float tfx = ((fx - c.ox) * c.ix) * 1.00000024f;
+  const float tfy = ((fy - c.oy) * c.iy) * 1.00000024f;
+  const float tfz = ((fz - c.oz) * c.iz) * 1.00000024f;
+  const float tmin = fmaxf(tnz, fmaxf(tny, fmaxf(tnx, min_t)));
+  const float tmax = fminf(tfz, fminf(tfy, fminf(tfx, max_t)));
+  return tmin <= tmax;
 }
 
 // Watertight test on a component-major triangle: VX = {A[kx] B[kx] C[kx] w} etc.  Arithmetic order of
@@ -137,6 +163,9 @@ constexpr int kNone3 = kEmptyLeaf;  // "no node": finished, or (with a non-empty
 
 constexpr int kTraverseBlock = 128;  // threads per CTA
 constexpr int kNodeExit = 8;         // leave the node phase when fewer lanes than this want node work
+// flags bit that only the counting launch sets (it clears the caller's): the tree is one leaf, and its root pair is the
+// leaf plus an empty phantom child that the reference never visits
+constexpr uint32_t kCountRootIsLeaf = 1u << 31;
 
 // Launch policy of traverse_fast3_kernel (the values and why: traverse.cu)
 template <int MINB_, int REFILL_MIN_, bool PAIR128_, int LEAF_AGAIN_MIN_, bool DEFER_RETIRE_, int NODE_UNROLL_>
@@ -185,6 +214,7 @@ __global__ void __launch_bounds__(kTraverseBlock, P::kMinBlocks)
   int cur = kNone3, leaf = kNone3;
   bool exhausted = false;
   unsigned long long n_boxes = 0, n_prims = 0;
+  const bool root_is_leaf = COUNT && (flags & kCountRootIsLeaf) != 0u;
   // COUNT only: lane-state histogram of the warp's iterations (nrt_traverse_lane_stats_device; lane 0 accumulates)
   unsigned long long st[14] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
 
@@ -222,7 +252,19 @@ __global__ void __launch_bounds__(kTraverseBlock, P::kMinBlocks)
           sp = 0;
           cur = range_has_nan(min_t, max_t) ? kNone3 : 0;
           leaf = kNone3;
-          if (COUNT) n_boxes += 1;
+          if (COUNT) {
+            // the reference's first pop, the root box; a ray that misses it visits nothing else
+            n_boxes += 1;
+            float4 X, Y, Z;
+            if (P::kPair128) {
+              X = __ldg(pair4 + c.nx);
+              Y = __ldg(pair4 + c.ny);
+              Z = __ldg(pair4 + c.nz);
+            } else {
+              wide_planes(c, __ldg(pair4), __ldg(pair4 + 1), __ldg(pair4 + 2), X, Y, Z);
+            }
+            if (cur == 0 && !slab_union(c, X, Y, Z, min_t, max_t)) cur = kNone3;
+          }
         }
       }
     }
@@ -283,7 +325,7 @@ __global__ void __launch_bounds__(kTraverseBlock, P::kMinBlocks)
               R = __ldg(reinterpret_cast<const int2 *>(q + 3));
               slab_pair_sel(c, q0, q1, q2, min_t, best.t, h0, h1, t0, t1);
             }
-            if (COUNT) n_boxes += 2;
+            if (COUNT) n_boxes += (root_is_leaf && cur == 0) ? 0 : 2;  // the one-leaf root was counted at load
             const bool swap = t1 < t0;
             const bool both = h0 & h1;
             if (both) {

@@ -21,9 +21,9 @@ def _rel(a, b, floor=1e-3):
     return float(np.max(np.abs(a - b) / np.maximum(np.abs(b), floor))) if a.size else 0.0
 
 
-def _setup(torch, api, S, v, f, mats, ids, emissive, fvn, W, H, spp, bounces, seed, camera="cornell"):
+def _setup(torch, api, S, v, f, mats, ids, emissive, fvn, W, H, spp, bounces, seed, camera="cornell", build_flags=0):
     acc = api.BVHAccel()
-    acc.Build(len(f), v, f)
+    acc.Build(len(f), v, f, flags=build_flags)
     keep = {"m": torch.as_tensor(np.ascontiguousarray(mats).view(np.float32).reshape(-1), device="cuda"),
             "i": torch.as_tensor(ids.astype(np.int32), device="cuda"),
             "e": torch.as_tensor(emissive.astype(np.int32), device="cuda"),
@@ -41,7 +41,7 @@ def _setup(torch, api, S, v, f, mats, ids, emissive, fvn, W, H, spp, bounces, se
     return acc, p, cam, keep
 
 
-def _bounce_by_bounce(with_normals, scene="cornell"):
+def _bounce_by_bounce(with_normals, scene="cornell", build_flags=0, min_depth=0):
     import torch
     from oracle import orc
     from nanort_b200 import api, dist as nd, scenes as S
@@ -62,7 +62,9 @@ def _bounce_by_bounce(with_normals, scene="cornell"):
     ref = orc.ReferencePathTracer(v, f, ids, mats)  # face normals as the example's loader makes them (calcNormal)
     assert np.array_equal(ref.emissive_faces(), emissive), "MeshLight's emissive-face list != the list handed to the device"
     fvn = ref.fvn if with_normals else None
-    acc, p, cam, keep = _setup(torch, api, S, v, f, mats, ids, emissive, fvn, W, H, spp, bounces, seed, camera=scene)
+    acc, p, cam, keep = _setup(torch, api, S, v, f, mats, ids, emissive, fvn, W, H, spp, bounces, seed, camera=scene,
+                               build_flags=build_flags)
+    assert acc.GetStatistics()["max_tree_depth"] >= min_depth
 
     # bounce 0 input: the camera rays of every slot (slot = path id), weight 1, do_emission = true
     pix_of_slot, smp_of_slot = nd.slot_pixels(W, H, TILE[0], TILE[1], 0, 1, spp)
@@ -179,6 +181,14 @@ def test_every_bounce_matches_the_reference_functions_on_the_1m_triangle_terrain
     """BASELINE.json configs[2]'s scene (terrain + area light, diffuse): the same per-bounce comparison with the reference's
     own shading code, at 2 spp on 192x108 pixels."""
     _bounce_by_bounce(with_normals=False, scene="terrain")
+
+
+def test_every_bounce_matches_the_reference_functions_on_the_reference_built_terrain():
+    """The same terrain from the reference-exact builder, a tree more than 200 levels deep: the radiance launch
+    (PathRadiancePolicy) and the shadow launches run with their 512-entry stacks."""
+    from nanort_b200 import api
+
+    _bounce_by_bounce(with_normals=False, scene="terrain", build_flags=api.BUILD_REFERENCE_TREE, min_depth=200)
 
 
 def test_whole_pass_equals_the_sum_of_its_bounces():
