@@ -58,7 +58,7 @@ def test_pass_fused_equals_unfused_and_matches_oracle(port, name, kw, W, H, spp)
     for s in range(spp):
         sel = valid & (smp == s)
         want[sel] = S.primary_rays(cam, W, H, spp=1, seed=1, pixels=pix[sel], sample0=s)
-    assert np.allclose(prim["dir"][valid], want["dir"][valid], atol=2e-7)
+    assert np.array_equal(prim["dir"][valid].view(np.uint32), want["dir"][valid].view(np.uint32))  # bit for bit
     assert np.array_equal(prim["org"][valid], want["org"][valid])
     assert np.all(prim["max_t"][~valid] < 0)
 
