@@ -231,7 +231,8 @@ static int traverse_small(Accel *a, const void *rays, size_t n, void *hits_16B, 
     char *hb = static_cast<char *>(sl.h);
     memcpy(hb, rays, n * ray_bytes);
     rc = launch_traverse(a, reinterpret_cast<const Ray36 *>(hb), n, reinterpret_cast<Hit16 *>(hb + off_hits),
-                         hit_mask ? reinterpret_cast<uint8_t *>(hb + off_mask) : nullptr, opt, flags, sl.s);
+                         hit_mask ? reinterpret_cast<uint8_t *>(hb + off_mask) : nullptr, opt, flags, sl.s,
+                         reinterpret_cast<unsigned long long *>(a->d_counters) + Accel::kSmallCursor0 + idx);
     e = cudaStreamSynchronize(sl.s);  // also on a failed launch: nothing of this call may be left in flight
     if (rc == NRT_OK && e == cudaSuccess) {
       memcpy(hits_16B, hb + off_hits, n * sizeof(Hit16));

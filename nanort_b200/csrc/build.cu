@@ -453,6 +453,12 @@ struct WarpSub {
   uint16_t tmp[kSubtree];
 };
 
+// One warp's slice of subtree_kernel's shared memory: WarpSub, B bin records, 2*B sweep floats -- rounded up to 16
+// bytes, because the next warp's WarpSub starts with float4 records (an odd bin_size would misalign them otherwise).
+__host__ __device__ constexpr size_t sub_slice_bytes(int B) {
+  return (sizeof(WarpSub) + (size_t)B * kBinWords * 4 + (size_t)2 * B * 4 + 15) & ~(size_t)15;
+}
+
 // Pool ids for one warp's subtree: reserved a chunk at a time (one atomic per chunk instead of one per split; the
 // pre-order indices are computed in closed form in phase C, so pool order is free).  A subtree of t primitives has at
 // most 2t - 2 nodes below its root and the reservations never exceed that, which keeps the whole pool within its 2n
@@ -984,8 +990,7 @@ __global__ void __launch_bounds__(kSubWarps * 32, 6)
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t sub = blockIdx.x * kSubWarps + warp;
   if (sub >= n_subtrees) return;
-  const size_t per_warp = sizeof(WarpSub) + (size_t)B * kBinWords * 4 + (size_t)2 * B * 4;
-  unsigned char *mine = smem_raw + (size_t)warp * per_warp;
+  unsigned char *mine = smem_raw + (size_t)warp * sub_slice_bytes(B);
   WarpSub &S = *reinterpret_cast<WarpSub *>(mine);
   uint32_t *sbin = reinterpret_cast<uint32_t *>(mine + sizeof(WarpSub));  // B*kBinWords: one axis at a time
   float *sweep = reinterpret_cast<float *>(sbin + (size_t)B * kBinWords);  // 2*B floats
@@ -1306,7 +1311,7 @@ int build_on_device(Accel *a, cudaStream_t s) {
   int cur = 0, which = 0;
   uint32_t n_active = 0;
   uint32_t n_nodes = 0;
-  const size_t sub_smem = kSubWarps * (sizeof(WarpSub) + (size_t)B * kBinWords * 4 + (size_t)2 * B * 4);
+  const size_t sub_smem = kSubWarps * sub_slice_bytes(B);
 
   BUILD_CUDA(cudaEventCreate(&ev0));
   BUILD_CUDA(cudaEventCreate(&ev1));

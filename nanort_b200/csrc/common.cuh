@@ -172,14 +172,19 @@ struct Accel {
     cudaStream_t s = nullptr;
     bool busy = false;
   };
+  // slot i launches with the ray cursor d_counters[kSmallCursor0 + i]: a slot is held until its launch has finished, so
+  // its cursor is never shared, however many calls other host threads make in the meantime
+  static constexpr int kSmallCursor0 = 80;
   SmallSlot small[kSmallSlots];
+  static_assert(kSmallCursor0 + kSmallSlots <= 96, "small-slot cursors lie inside d_counters");
   std::mutex small_mu;
   std::condition_variable small_cv;
   // wavefront pass scratch (render.cu)
   void *d_wave = nullptr;
   size_t wave_bytes = 0;
-  // device counter block: [0..7] misc, [8..9] visit counts, [16..47] ring of ray cursors (one per
-  // in-flight traversal launch, so launches on different streams never share a cursor)
+  // device counter block (96 words): [0..7] misc, [8..9] visit counts, [16..47] ring of ray cursors (one per
+  // in-flight traversal launch, so launches on different streams never share a cursor), [48..54] path tracer,
+  // [64..79] count / lane-stat scratch, [80..95] the small slots' ray cursors
   uint64_t *d_counters = nullptr;
   mutable std::atomic<uint32_t> cursor_ring{0};
 };
@@ -248,8 +253,10 @@ inline BuildOptions28 default_build_options() {
 
 // ---- kernels / stages implemented in the other translation units -------------------
 // traverse.cu
+// `cursor`: the persistent kernel's ray cursor (a device word, zeroed on `s` before the launch); nullptr takes the
+// next one of the accel's ring
 int launch_traverse(const Accel *a, const Ray36 *d_rays, size_t n, Hit16 *d_hits, uint8_t *d_mask,
-                    const TraceOptions16 &opt, uint32_t flags, cudaStream_t s);
+                    const TraceOptions16 &opt, uint32_t flags, cudaStream_t s, unsigned long long *cursor = nullptr);
 int launch_traverse_count(const Accel *a, const Ray36 *d_rays, size_t n, const TraceOptions16 &opt,
                           uint32_t flags, uint64_t *d_counts2, cudaStream_t s);
 // SoA wavefront entry used by render.cu: rays as two float4 (org.xyz,min_t | dir.xyz,max_t)

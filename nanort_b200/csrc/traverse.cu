@@ -198,7 +198,8 @@ constexpr size_t kPair128MaxBytes = (size_t)38 << 20;
 
 static unsigned long long *next_cursor(const Accel *a, cudaStream_t s, cudaError_t *e) {
   // ring of 32 cursors: launches in flight on different streams never share one.  More than 32 traversal launches
-  // of ONE accel in flight at once would alias; every entry point of this library keeps at most 3.
+  // of ONE accel in flight at once would alias; every entry point that draws from the ring keeps at most 3 (the
+  // small-call path, which many host threads use at once, has one cursor per slot instead: Accel::kSmallCursor0).
   unsigned long long *cursor =
       reinterpret_cast<unsigned long long *>(a->d_counters) + 16 + (a->cursor_ring.fetch_add(1) & 31u);
   *e = cudaMemsetAsync(cursor, 0, sizeof(unsigned long long), s);
@@ -228,13 +229,17 @@ static bool needs_deep_stack(const Accel *a) { return a->stats.max_tree_depth + 
 
 template <class Rays, bool COUNT, class P, class Epi>
 static int launch_fast3_any(const Accel *a, Rays rays, size_t n, Epi epi, const TraceOptions16 &opt, uint32_t flags,
-                            unsigned long long *d_counts, const unsigned long long *n_ptr, cudaStream_t s) {
+                            unsigned long long *d_counts, const unsigned long long *n_ptr, cudaStream_t s,
+                            unsigned long long *cursor = nullptr) {
   if (!a->d_pair || !a->d_tris_cm) {
     set_error("traverse: this accel has no triangle traversal layout");
     return NRT_ERR_INVALID;
   }
   cudaError_t e;
-  unsigned long long *cursor = next_cursor(a, s, &e);
+  if (cursor)
+    e = cudaMemsetAsync(cursor, 0, sizeof(unsigned long long), s);
+  else
+    cursor = next_cursor(a, s, &e);
   NRT_CUDA(e);
   if (needs_deep_stack(a))
     e = launch_fast3<Rays, 512, COUNT, P>(a, rays, n, epi, opt, flags, cursor, d_counts, n_ptr, s);
@@ -247,22 +252,23 @@ static int launch_fast3_any(const Accel *a, Rays rays, size_t n, Epi epi, const 
 // the default for coherent launches, with the size cut-off
 template <class Rays, bool COUNT, class Epi>
 static int launch_fast3_coherent(const Accel *a, Rays rays, size_t n, Epi epi, const TraceOptions16 &opt, uint32_t flags,
-                                 unsigned long long *d_counts, const unsigned long long *n_ptr, cudaStream_t s) {
+                                 unsigned long long *d_counts, const unsigned long long *n_ptr, cudaStream_t s,
+                                 unsigned long long *cursor = nullptr) {
   if (a->n_wide * sizeof(PairNode) > kPair128MaxBytes)
-    return launch_fast3_any<Rays, COUNT, IncoherentPolicy>(a, rays, n, epi, opt, flags, d_counts, n_ptr, s);
-  return launch_fast3_any<Rays, COUNT, DefaultPolicy>(a, rays, n, epi, opt, flags, d_counts, n_ptr, s);
+    return launch_fast3_any<Rays, COUNT, IncoherentPolicy>(a, rays, n, epi, opt, flags, d_counts, n_ptr, s, cursor);
+  return launch_fast3_any<Rays, COUNT, DefaultPolicy>(a, rays, n, epi, opt, flags, d_counts, n_ptr, s, cursor);
 }
 
 template <class Rays, bool COUNT>
 static int launch_fast(const Accel *a, Rays rays, size_t n, Hit16 *d_hits, uint8_t *d_mask,
                        const TraceOptions16 &opt, uint32_t flags, unsigned long long *d_counts, cudaStream_t s,
-                       const unsigned long long *n_ptr = nullptr) {
+                       const unsigned long long *n_ptr = nullptr, unsigned long long *cursor = nullptr) {
   if (!COUNT && ((flags >> 8) & 0xFFu) != 0) {  // the counting walk ignores them
     set_error("nrt_traverse: flags bits 8..15 are reserved");
     return NRT_ERR_INVALID;
   }
   const StoreHitsEpilogue epi{d_hits, d_mask};
-  return launch_fast3_coherent<Rays, COUNT>(a, rays, n, epi, opt, flags, d_counts, n_ptr, s);
+  return launch_fast3_coherent<Rays, COUNT>(a, rays, n, epi, opt, flags, d_counts, n_ptr, s, cursor);
 }
 
 template <class Rays, bool COUNT>
@@ -278,7 +284,7 @@ static int launch_conf(const Accel *a, Rays rays, size_t n, Hit16 *d_hits, uint8
 }
 
 int launch_traverse(const Accel *a, const Ray36 *d_rays, size_t n, Hit16 *d_hits, uint8_t *d_mask,
-                    const TraceOptions16 &opt, uint32_t flags, cudaStream_t s) {
+                    const TraceOptions16 &opt, uint32_t flags, cudaStream_t s, unsigned long long *cursor) {
   if (n == 0) return NRT_OK;
   if (flags & NRT_TRAVERSE_RAY32) {  // compact records: default policy only
     if (a->prim_kind != 0 || (reinterpret_cast<uintptr_t>(d_rays) & 15u) != 0) {
@@ -290,16 +296,17 @@ int launch_traverse(const Accel *a, const Ray36 *d_rays, size_t n, Hit16 *d_hits
       return launch_conf<Aos32Rays, false>(a, r32, n, d_hits, d_mask, opt, flags, nullptr, s);
     const StoreHitsEpilogue epi{d_hits, d_mask};
     if (flags & NRT_TRAVERSE_ANY_HIT)
-      return launch_fast3_coherent<Aos32Rays, false>(a, r32, n, AnyHit<StoreHitsEpilogue>(epi), opt, flags, nullptr, nullptr, s);
-    return launch_fast3_coherent<Aos32Rays, false>(a, r32, n, epi, opt, flags, nullptr, nullptr, s);
+      return launch_fast3_coherent<Aos32Rays, false>(a, r32, n, AnyHit<StoreHitsEpilogue>(epi), opt, flags, nullptr, nullptr, s,
+                                                     cursor);
+    return launch_fast3_coherent<Aos32Rays, false>(a, r32, n, epi, opt, flags, nullptr, nullptr, s, cursor);
   }
   if (a->prim_kind != 0) return launch_traverse_prims(a, d_rays, n, d_hits, d_mask, opt, flags, s);  // spheres ...
   AosRays r{d_rays};
   if (flags & NRT_TRAVERSE_CONFORMANCE) return launch_conf<AosRays, false>(a, r, n, d_hits, d_mask, opt, flags, nullptr, s);
   if (flags & NRT_TRAVERSE_ANY_HIT)  // occlusion query: default policy only
     return launch_fast3_coherent<AosRays, false>(a, r, n, AnyHit<StoreHitsEpilogue>(StoreHitsEpilogue{d_hits, d_mask}), opt,
-                                                 flags, nullptr, nullptr, s);
-  return launch_fast<AosRays, false>(a, r, n, d_hits, d_mask, opt, flags, nullptr, s);
+                                                 flags, nullptr, nullptr, s, cursor);
+  return launch_fast<AosRays, false>(a, r, n, d_hits, d_mask, opt, flags, nullptr, s, nullptr, cursor);
 }
 
 int launch_traverse_soa(const Accel *a, const float4 *d_org_tmin, const float4 *d_dir_tmax, size_t n,

@@ -104,3 +104,40 @@ def check_tree_structure(nodes, indices, verts, faces, min_leaf=4, max_depth=256
     # boxes are the exact float min/max of the member triangles (numerically: -0.0 == 0.0)
     assert np.array_equal(nodes["bmin"], bmin) and np.array_equal(nodes["bmax"], bmax), "exact node boxes"
     return {"max_tree_depth": int(depth.max()), "num_leaf_nodes": n_leaf, "num_branch_nodes": n_branch}
+
+
+def random_soup(rng, n):
+    """Clustered triangle soup: cluster centres on very different scales, many coincident centroids, some slivers."""
+    k = int(rng.integers(1, 6))
+    centres = rng.normal(0, 10.0 ** rng.uniform(-2, 2), (k, 3))
+    which = rng.integers(0, k, n)
+    spread = 10.0 ** rng.uniform(-3, 0.5, k)
+    c = centres[which] + rng.normal(0, 1, (n, 3)) * spread[which][:, None]
+    dup = rng.random(n) < 0.15  # exact duplicates of another triangle's centroid position
+    c[dup] = c[rng.integers(0, n, int(dup.sum()))]
+    size = 10.0 ** rng.uniform(-3, 0, (n, 1, 1))
+    tri = c[:, None, :] + rng.normal(0, 1, (n, 3, 3)) * size
+    flat = rng.random(n) < 0.1  # axis-aligned flat triangles: zero-thickness boxes
+    tri[flat, :, int(rng.integers(0, 3))] = c[flat, int(rng.integers(0, 3))][:, None]
+    v = tri.reshape(-1, 3).astype(np.float32)
+    return v, np.arange(3 * n, dtype=np.uint32).reshape(n, 3)
+
+
+def degenerate_mesh(kind):
+    """Small or degenerate triangle sets: one triangle, five, 3000 copies of one, 700 centroids on a line."""
+    if kind == "one":
+        v = np.array([[0, 0, 0], [1, 0, 0], [0, 1, 0]], np.float32)
+        return v, np.array([[0, 1, 2]], np.uint32)
+    if kind == "five":
+        v = np.array([[0, 0, 0], [1, 0, 0], [0, 1, 0], [2, 0, 1], [3, 1, 1], [2, 2, 2], [5, 5, 5]], np.float32)
+        return v, np.array([[0, 1, 2], [1, 2, 3], [2, 3, 4], [3, 4, 5], [4, 5, 6]], np.uint32)
+    if kind == "identical":  # 3000 copies of one triangle: no plane separates the centroids -> median cuts
+        v = np.array([[0, 0, 0], [1, 0, 0], [0, 1, 0]], np.float32)
+        return v, np.tile(np.array([[0, 1, 2]], np.uint32), (3000, 1))
+    if kind == "line":  # centroids on a line along x only
+        k = 700
+        x = np.arange(k, dtype=np.float32)
+        v = np.stack([np.stack([x, 0 * x, 0 * x], 1), np.stack([x + 0.5, 0 * x, 0 * x + 1], 1),
+                      np.stack([x, 0 * x + 1, 0 * x], 1)], 1).reshape(-1, 3)
+        return v.astype(np.float32), np.arange(3 * k, dtype=np.uint32).reshape(k, 3)
+    raise KeyError(kind)

@@ -2,28 +2,9 @@
 import numpy as np
 import pytest
 
-from helpers import assert_parity, check_tree_structure, compare_hits
+from helpers import assert_parity, check_tree_structure, compare_hits, degenerate_mesh, random_soup
 
 pytestmark = pytest.mark.gpu
-
-
-def _degenerate(kind):
-    if kind == "one":
-        v = np.array([[0, 0, 0], [1, 0, 0], [0, 1, 0]], np.float32)
-        return v, np.array([[0, 1, 2]], np.uint32)
-    if kind == "five":
-        v = np.array([[0, 0, 0], [1, 0, 0], [0, 1, 0], [2, 0, 1], [3, 1, 1], [2, 2, 2], [5, 5, 5]], np.float32)
-        return v, np.array([[0, 1, 2], [1, 2, 3], [2, 3, 4], [3, 4, 5], [4, 5, 6]], np.uint32)
-    if kind == "identical":  # 3000 copies of one triangle: no plane separates the centroids -> median cuts
-        v = np.array([[0, 0, 0], [1, 0, 0], [0, 1, 0]], np.float32)
-        return v, np.tile(np.array([[0, 1, 2]], np.uint32), (3000, 1))
-    if kind == "line":  # centroids on a line along x only
-        k = 700
-        x = np.arange(k, dtype=np.float32)
-        v = np.stack([np.stack([x, 0 * x, 0 * x], 1), np.stack([x + 0.5, 0 * x, 0 * x + 1], 1),
-                      np.stack([x, 0 * x + 1, 0 * x], 1)], 1).reshape(-1, 3)
-        return v.astype(np.float32), np.arange(3 * k, dtype=np.uint32).reshape(k, 3)
-    raise KeyError(kind)
 
 
 CASES = [
@@ -50,7 +31,7 @@ def _scene(name, kw):
     from nanort_b200 import scenes as S
 
     if name.startswith("deg:"):
-        return _degenerate(name[4:])
+        return degenerate_mesh(name[4:])
     return S.make_scene(name, **kw)
 
 
@@ -133,23 +114,6 @@ def test_reference_traverses_gpu_built_tree(reference, port):
     assert_parity(compare_hits(port, v, f, rays, got_h, got_m, want_h, want_m))
 
 
-def _random_soup(rng, n):
-    """Clustered triangle soup: cluster centres on very different scales, many coincident centroids, some slivers."""
-    k = int(rng.integers(1, 6))
-    centres = rng.normal(0, 10.0 ** rng.uniform(-2, 2), (k, 3))
-    which = rng.integers(0, k, n)
-    spread = 10.0 ** rng.uniform(-3, 0.5, k)
-    c = centres[which] + rng.normal(0, 1, (n, 3)) * spread[which][:, None]
-    dup = rng.random(n) < 0.15  # exact duplicates of another triangle's centroid position
-    c[dup] = c[rng.integers(0, n, int(dup.sum()))]
-    size = 10.0 ** rng.uniform(-3, 0, (n, 1, 1))
-    tri = c[:, None, :] + rng.normal(0, 1, (n, 3, 3)) * size
-    flat = rng.random(n) < 0.1  # axis-aligned flat triangles: zero-thickness boxes
-    tri[flat, :, int(rng.integers(0, 3))] = c[flat, int(rng.integers(0, 3))][:, None]
-    v = tri.reshape(-1, 3).astype(np.float32)
-    return v, np.arange(3 * n, dtype=np.uint32).reshape(n, 3)
-
-
 @pytest.mark.parametrize("seed", range(24))
 def test_random_soups_and_options(port, seed):
     """Sizes around every class boundary of the builder (one warp-built subtree <= 128 < one-CTA node <= 2048 <
@@ -161,7 +125,7 @@ def test_random_soups_and_options(port, seed):
     rng = np.random.default_rng(1000 + seed)
     sizes = [2, 5, 31, 33, 64, 127, 128, 129, 400, 1000, 2047, 2048, 2049, 3000, 5000, 9000]
     n = sizes[seed % len(sizes)] if seed < 16 else int(rng.integers(2, 12000))
-    v, f = _random_soup(rng, n)
+    v, f = random_soup(rng, n)
     okw = dict(min_leaf_primitives=int(rng.choice([1, 1, 2, 4, 4, 8, 13])), bin_size=int(rng.choice([2, 4, 8, 16, 64, 64, 128])),
                max_tree_depth=int(rng.choice([3, 8, 20, 256, 256])))
     opts = api.BVHBuildOptions(**okw)
