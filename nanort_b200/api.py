@@ -590,6 +590,9 @@ class Scene:
         return hits, mask
 
     def TraverseDevice(self, d_rays_ptr, n, d_hits_ptr, d_mask_ptr=None, flags=TRAVERSE_FAST, stream=None):
+        """Asynchronous on `stream`.  Any number of calls (and scene AO passes) on one scene may be in flight on any
+        streams at once: a call is ordered on the device after the earlier call that used the same one of the
+        scene's four scratch sets; the host does not wait."""
         _check(lib().nrt_scene_traverse_device(self._h, C.c_void_p(d_rays_ptr), int(n), C.c_void_p(d_hits_ptr),
                                                C.c_void_p(d_mask_ptr) if d_mask_ptr else None, int(flags),
                                                C.c_void_p(stream) if stream else None))

@@ -547,8 +547,11 @@ __global__ void __launch_bounds__(kSceneBlock, MINB)
         float t0, t1;
         bool h0 = slab_e(c, q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, lo_clip, hi_clip, t0);
         bool h1 = slab_e(c, q1.z, q1.w, q2.x, q2.y, q2.z, q2.w, lo_clip, hi_clip, t1);
-        h0 &= !(t0 > bound);
-        h1 &= !(t1 > bound);
+        // an empty child (the second child of a root that is a leaf) never passes: its inverted box does pass when
+        // the ray's origin is NaN, because slab_e drops NaN operands, and kNoLeaf as the next node inside an
+        // instance would leave the lane there for ever
+        h0 &= !(t0 > bound) && q3.x != kNoLeaf;
+        h1 &= !(t1 > bound) && q3.y != kNoLeaf;
         const bool both = h0 & h1;
         const bool swap = t1 < t0;
         const int nearr = swap ? q3.y : q3.x;
@@ -674,13 +677,16 @@ struct Scene {
   InstanceDev *d_inst = nullptr;
   float *d_state = nullptr;  // 76 floats per instance
   uint32_t max_blas_depth = 0;
-  // per-launch scratch, handed out round-robin so that traversals in flight on different streams never share it:
-  // slot k owns the ray cursor d_counters[k], the overflow count d_counters[4 + k] and its own overflow list
+  // per-launch scratch, handed out round-robin: slot k owns the ray cursor d_counters[k], the overflow count
+  // d_counters[4 + k] and its own overflow list.  slot_done[k] is recorded after the last launch that used slot k,
+  // and the next launch on slot k makes its stream wait for it, so launches in flight on any number of streams never
+  // share a cursor or an overflow list.  next_slot and the events are guarded by mu.
   static constexpr int kSlots = 4;
   uint32_t *d_overflow[kSlots] = {nullptr, nullptr, nullptr, nullptr};
   size_t overflow_cap[kSlots] = {0, 0, 0, 0};
+  cudaEvent_t slot_done[kSlots] = {nullptr, nullptr, nullptr, nullptr};
   unsigned long long *d_counters = nullptr;
-  std::atomic<uint32_t> ring{0};
+  uint32_t next_slot = 0;
   cudaStream_t stream = nullptr;
   void *d_rays = nullptr, *d_hits = nullptr, *d_mask = nullptr;
   size_t stage = 0;
@@ -700,7 +706,10 @@ static void scene_destroy(Scene *s) {
   }
   cudaFree(s->d_inst);
   cudaFree(s->d_state);
-  for (int k = 0; k < Scene::kSlots; k++) cudaFree(s->d_overflow[k]);
+  for (int k = 0; k < Scene::kSlots; k++) {
+    cudaFree(s->d_overflow[k]);
+    if (s->slot_done[k]) cudaEventDestroy(s->slot_done[k]);
+  }
   cudaFree(s->d_counters);
   cudaFree(s->d_rays);
   cudaFree(s->d_hits);
@@ -730,19 +739,21 @@ static int scene_launch(Scene *sc, const Ray36 *d_rays, size_t n, SceneHit32 *d_
     set_error("nrt_scene_traverse: flags bits 8..15 are reserved");
     return NRT_ERR_INVALID;
   }
-  const int slot = (int)(sc->ring.fetch_add(1) % (uint32_t)Scene::kSlots);
-  uint32_t *d_overflow = nullptr;
-  {
-    std::lock_guard<std::mutex> lock(sc->mu);
-    if (sc->overflow_cap[slot] < n) {  // grows rarely; cudaFree waits for launches still using the old list
-      cudaFree(sc->d_overflow[slot]);
-      sc->d_overflow[slot] = nullptr;
-      sc->overflow_cap[slot] = 0;
-      NRT_CUDA(cudaMalloc(&sc->d_overflow[slot], sizeof(uint32_t) * n));
-      sc->overflow_cap[slot] = n;
-    }
-    d_overflow = sc->d_overflow[slot];
+  // the whole launch sequence under the lock: taking the slot, waiting for its previous user, enqueueing the kernels
+  // and recording slot_done happen in the same order on the host and on the device
+  std::lock_guard<std::mutex> lock(sc->mu);
+  const int slot = (int)sc->next_slot;
+  sc->next_slot = (sc->next_slot + 1) % (uint32_t)Scene::kSlots;
+  if (sc->overflow_cap[slot] < n) {  // grows rarely; the launch that last used the old list must be done with it
+    NRT_CUDA(cudaEventSynchronize(sc->slot_done[slot]));
+    cudaFree(sc->d_overflow[slot]);
+    sc->d_overflow[slot] = nullptr;
+    sc->overflow_cap[slot] = 0;
+    NRT_CUDA(cudaMalloc(&sc->d_overflow[slot], sizeof(uint32_t) * n));
+    sc->overflow_cap[slot] = n;
   }
+  uint32_t *d_overflow = sc->d_overflow[slot];
+  NRT_CUDA(cudaStreamWaitEvent(s, sc->slot_done[slot], 0));
   unsigned long long *cursor = sc->d_counters + slot;
   unsigned long long *ovf = sc->d_counters + Scene::kSlots + slot;
   NRT_CUDA(cudaMemsetAsync(cursor, 0, sizeof(unsigned long long), s));
@@ -760,6 +771,7 @@ static int scene_launch(Scene *sc, const Ray36 *d_rays, size_t n, SceneHit32 *d_
   scene_list_kernel<<<(unsigned)std::min<size_t>((n + 127) / 128, (size_t)sms * 4), 128, 0, s>>>(
       dev, d_rays, n, d_overflow, ovf, d_hits, d_mask, flags);
   NRT_CUDA(cudaGetLastError());
+  NRT_CUDA(cudaEventRecord(sc->slot_done[slot], s));
   return NRT_OK;
 }
 
@@ -806,6 +818,8 @@ int nrt_scene_commit(const nrt_instance *instances, uint32_t n_instances, uint32
   if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&sc->stream, cudaStreamNonBlocking);
   if (e == cudaSuccess) e = cudaMalloc(&sc->d_counters, 32 * sizeof(unsigned long long));
   if (e == cudaSuccess) e = cudaMemset(sc->d_counters, 0, 32 * sizeof(unsigned long long));
+  for (int k = 0; k < Scene::kSlots && e == cudaSuccess; k++)
+    e = cudaEventCreateWithFlags(&sc->slot_done[k], cudaEventDisableTiming);
   if (e == cudaSuccess) e = cudaMalloc(&sc->d_inst, sizeof(InstanceDev) * (size_t)n_instances);
   if (e == cudaSuccess) e = cudaMalloc(&sc->d_state, sizeof(float) * 76 * (size_t)n_instances);
   if (e == cudaSuccess) e = cudaMalloc(&d_in, sizeof(InstanceIn) * (size_t)n_instances);
@@ -908,6 +922,8 @@ int nrt_scene_instance_state(const nrt_scene *s, uint32_t instance, float out76[
   return NRT_OK;
 }
 
+// Asynchronous on `stream`.  Any number of calls (and scene AO passes) on one scene may be in flight on any streams at
+// once: scene_launch orders a call on the device after the earlier call that used the same scratch slot.
 int nrt_scene_traverse_device(const nrt_scene *s, const void *d_rays_36B, size_t n_rays, void *d_hits_32B,
                               uint8_t *d_hit_mask, uint32_t flags, void *stream) {
   if (!s || (n_rays && (!d_rays_36B || !d_hits_32B))) {

@@ -872,6 +872,8 @@ int orc_test_prim(const real *verts, size_t stride, const uint32_t *faces, const
  *   orc_sg_list                BVHAccel::ListNodeIntersections + TestLeafNodeIntersections with
  *                              NodeBBoxIntersector                      nanort.h:2558-2692, nanosg.h:592-660
  *   orc_sg_traverse_one        Scene::Traverse                          nanosg.h:779-875
+ *   orc_sg_instance_hit        its per-instance body                    nanosg.h:831-850
+ *   orc_sg_prim_hit            the same body on one triangle (tie re-tests, no reference counterpart)
  * Parity status: PINNED against oracle/_ref/libnanosg_ref*.so (tests/test_oracle_scene.py).
  *
  * Reference behaviours restated as they are (none is "fixed" here):
@@ -1106,42 +1108,78 @@ int orc_sg_list(const orc_node *top, const uint32_t *top_idx, const orc_sg_node 
   return n;
 }
 
+/* One instance of Scene::Traverse (nanosg.h:831-850): the world ray moved into instance `id` (MultV with inv and
+ * inv33), the local ray {0, FLT_MAX} walked through the instance's tree -- or, for prim != 0xFFFFFFFF, tested against
+ * that one triangle alone -- then the local hit point moved back to world space and its distance from the world
+ * origin.  Returns 1 and the whole record on a hit. */
+static int sg_local_hit(const orc_sg_node *sg, const orc_sg_blas *blas, const orc_ray *ray, uint32_t id, uint32_t prim,
+                        int cpp11, orc_sg_hit *hit) {
+  const orc_sg_node *nd = &sg[id];
+  const orc_sg_blas *b = &blas[id];
+  orc_ray lr;
+  orc_multv(lr.org, nd->inv, ray->org);
+  orc_multv(lr.dir, nd->inv33, ray->dir);
+  lr.min_t = 0.0f;
+  lr.max_t = FLT_MAX;
+  lr.type = 0;
+  orc_hit lh;
+  if (prim == 0xFFFFFFFFu) {
+    if (!orc_traverse_one(b->nodes, b->indices, b->verts, b->stride, b->faces, &lr, NULL, cpp11, &lh, NULL)) return 0;
+  } else if (!orc_test_prim(b->verts, b->stride, b->faces, &lr, NULL, cpp11, prim, &lh)) {
+    return 0;
+  }
+  float lp[3], wp[3];
+  for (int k = 0; k < 3; k++) lp[k] = lr.org[k] + lh.t * lr.dir[k];
+  orc_multv(wp, nd->xform, lp);
+  const float px = wp[0] - ray->org[0], py = wp[1] - ray->org[1], pz = wp[2] - ray->org[2];
+  hit->u = lh.u;
+  hit->v = lh.v;
+  hit->t = sqrtf((px * px + py * py) + pz * pz);
+  hit->prim_id = lh.prim_id;
+  hit->node_id = id;
+  hit->P[0] = wp[0];
+  hit->P[1] = wp[1];
+  hit->P[2] = wp[2];
+  return 1;
+}
+
+/* the nearest hit inside instance `id` alone, as Scene::Traverse records it */
+int orc_sg_instance_hit(const orc_sg_node *sg, const orc_sg_blas *blas, const orc_ray *ray, uint32_t id, int cpp11,
+                        orc_sg_hit *hit) {
+  return sg_local_hit(sg, blas, ray, id, 0xFFFFFFFFu, cpp11, hit);
+}
+
+/* the record Scene::Traverse would write if triangle `prim` of instance `id` were its pick (tie re-tests) */
+int orc_sg_prim_hit(const orc_sg_node *sg, const orc_sg_blas *blas, const orc_ray *ray, uint32_t id, uint32_t prim,
+                    int cpp11, orc_sg_hit *hit) {
+  return sg_local_hit(sg, blas, ray, id, prim, cpp11, hit);
+}
+
+/* orc_sg_instance_hit (prims == NULL) or orc_sg_prim_hit for rays[i] and ids[i] / prims[i]; ok[i] = hit */
+void orc_sg_local_hit_batch(const orc_sg_node *sg, const orc_sg_blas *blas, const orc_ray *rays, size_t n,
+                            const uint32_t *ids, const uint32_t *prims, int cpp11, orc_sg_hit *hits, uint8_t *ok) {
+  for (size_t i = 0; i < n; i++)
+    ok[i] = (uint8_t)sg_local_hit(sg, blas, &rays[i], ids[i], prims ? prims[i] : 0xFFFFFFFFu, cpp11, &hits[i]);
+}
+
+/* Scene::Traverse with the node-hit list cut at max_hits boxes (the reference's kMaxIntersections = 64; at most 128) */
 int orc_sg_traverse_one(const orc_node *top, const uint32_t *top_idx, const orc_sg_node *sg,
-                        const orc_sg_blas *blas, const orc_ray *ray, int cpp11, orc_sg_hit *hit) {
+                        const orc_sg_blas *blas, const orc_ray *ray, int max_hits, int cpp11, orc_sg_hit *hit) {
   float tmin[128];
   uint32_t ids[128];
-  const int n = orc_sg_list(top, top_idx, sg, ray, 64, cpp11, tmin, NULL, ids);
+  if (max_hits < 1) max_hits = 1;
+  if (max_hits > 128) max_hits = 128;
+  const int n = orc_sg_list(top, top_idx, sg, ray, max_hits, cpp11, tmin, NULL, ids);
   float t_nearest = FLT_MAX;
   int has_hit = 0;
   for (int i = 0; i < n; i++) {
     if (t_nearest < tmin[i]) continue;
-    const orc_sg_node *nd = &sg[ids[i]];
-    const orc_sg_blas *b = &blas[ids[i]];
-    orc_ray lr;
-    orc_multv(lr.org, nd->inv, ray->org);
-    orc_multv(lr.dir, nd->inv33, ray->dir);
-    lr.min_t = 0.0f;
-    lr.max_t = FLT_MAX;
-    lr.type = 0;
-    orc_hit lh;
-    if (!orc_traverse_one(b->nodes, b->indices, b->verts, b->stride, b->faces, &lr, NULL, cpp11, &lh, NULL))
-      continue;
-    float lp[3], wp[3];
-    for (int k = 0; k < 3; k++) lp[k] = lr.org[k] + lh.t * lr.dir[k];
-    orc_multv(wp, nd->xform, lp);
-    const float px = wp[0] - ray->org[0], py = wp[1] - ray->org[1], pz = wp[2] - ray->org[2];
-    const float t_world = sqrtf((px * px + py * py) + pz * pz);
-    if (t_world < t_nearest) {
-      t_nearest = t_world;
+    orc_sg_hit h;
+    if (!sg_local_hit(sg, blas, ray, ids[i], 0xFFFFFFFFu, cpp11, &h)) continue;
+    if (h.t < t_nearest) {
+      t_nearest = h.t;
       has_hit = 1;
-      hit->u = lh.u;
-      hit->v = lh.v;
-      hit->t = t_world;
-      hit->prim_id = lh.prim_id;
-      hit->node_id = ids[i];
-      hit->P[0] = wp[0];
-      hit->P[1] = wp[1];
-      hit->P[2] = wp[2];
+      *hit = h;
     }
   }
   return has_hit;
@@ -1156,6 +1194,7 @@ typedef struct {
   size_t n_rays;
   orc_sg_hit *hits;
   uint8_t *mask;
+  int max_hits;
   int cpp11;
   size_t *next;
   pthread_mutex_t *mu;
@@ -1173,7 +1212,7 @@ static void *sg_worker(void *arg) {
     size_t e = b + 256 < j->n_rays ? b + 256 : j->n_rays;
     for (size_t i = b; i < e; i++) {
       orc_sg_hit h;
-      int hit = orc_sg_traverse_one(j->top, j->top_idx, j->sg, j->blas, &j->rays[i], j->cpp11, &h);
+      int hit = orc_sg_traverse_one(j->top, j->top_idx, j->sg, j->blas, &j->rays[i], j->max_hits, j->cpp11, &h);
       if (hit) {
         j->hits[i] = h;
         j->n_hits++;
@@ -1187,7 +1226,7 @@ static void *sg_worker(void *arg) {
 /* Scene::Traverse over a batch; hits[i] is written only where mask[i] == 1 */
 size_t orc_sg_traverse_batch(const orc_node *top, const uint32_t *top_idx, const orc_sg_node *sg,
                              const orc_sg_blas *blas, const orc_ray *rays, size_t n_rays, orc_sg_hit *hits,
-                             uint8_t *mask, int cpp11, int n_threads) {
+                             uint8_t *mask, int max_hits, int cpp11, int n_threads) {
   if (n_threads < 1) n_threads = 1;
   if (n_threads > 256) n_threads = 256;
   pthread_mutex_t mu = PTHREAD_MUTEX_INITIALIZER;
@@ -1195,7 +1234,7 @@ size_t orc_sg_traverse_batch(const orc_node *top, const uint32_t *top_idx, const
   sg_job jobs[256];
   pthread_t th[256];
   for (int t = 0; t < n_threads; t++) {
-    sg_job j = {top, top_idx, sg, blas, rays, n_rays, hits, mask, cpp11, &next, &mu, 0};
+    sg_job j = {top, top_idx, sg, blas, rays, n_rays, hits, mask, max_hits, cpp11, &next, &mu, 0};
     jobs[t] = j;
   }
   if (n_threads == 1) {

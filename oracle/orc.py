@@ -292,7 +292,10 @@ class PortScene:
                                   C.c_void_p, C.c_void_p]
         L.orc_sg_traverse_batch.restype = C.c_size_t
         L.orc_sg_traverse_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
-                                            C.c_void_p, C.c_void_p, C.c_int, C.c_int]
+                                            C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
+        L.orc_sg_local_hit_batch.restype = None
+        L.orc_sg_local_hit_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                             C.c_int, C.c_void_p, C.c_void_p]
         self.cpp11 = cpp11
         mode = MODE_CPP11 if cpp11 else 0
         n = len(instances)
@@ -323,21 +326,57 @@ class PortScene:
         self.top = np.frombuffer((C.c_char * (nn * 40)).from_address(out.value), NODE_DTYPE).copy()
         L.orc_free(out)
 
-    def list_node_intersections(self, ray, max_hits=64):
+    def _top(self, top, top_idx):
+        """this scene's own top-level tree, or any other one built over the same instance boxes (e.g. the tree a
+        device Commit produced, Scene.GetTopLevel())"""
+        if top is None:
+            return self.top, self.top_idx
+        top, top_idx = np.ascontiguousarray(top), np.ascontiguousarray(top_idx, np.uint32)
+        assert top.dtype.itemsize == 40 and len(top_idx) == len(self.sg)
+        return top, top_idx
+
+    def list_node_intersections(self, ray, max_hits=64, top=None, top_idx=None):
+        top, top_idx = self._top(top, top_idx)
         ray = np.ascontiguousarray(ray).reshape(1)
         tmin, tmax, ids = np.zeros(128, np.float32), np.zeros(128, np.float32), np.zeros(128, np.uint32)
-        n = self.port.lib.orc_sg_list(_p(self.top), _p(self.top_idx), _p(self.sg), _p(ray), max_hits,
+        n = self.port.lib.orc_sg_list(_p(top), _p(top_idx), _p(self.sg), _p(ray), max_hits,
                                       1 if self.cpp11 else 0, _p(tmin), _p(tmax), _p(ids))
         return tmin[:n], tmax[:n], ids[:n]
 
-    def traverse(self, rays, threads=1):
+    def traverse(self, rays, threads=1, top=None, top_idx=None, max_hits=64):
+        """Scene::Traverse over `top` (default: this scene's own top-level tree); max_hits (<= 128) replaces the
+        reference's 64-box limit."""
+        assert 1 <= max_hits <= 128
+        top, top_idx = self._top(top, top_idx)
         rays = np.ascontiguousarray(rays)
         n = len(rays)
         hits, mask = np.zeros(n, SG_HIT_DTYPE), np.zeros(n, np.uint8)
-        self.port.lib.orc_sg_traverse_batch(_p(self.top), _p(self.top_idx), _p(self.sg),
+        self.port.lib.orc_sg_traverse_batch(_p(top), _p(top_idx), _p(self.sg),
                                             C.addressof(self._blas_c), _p(rays), n, _p(hits), _p(mask),
-                                            1 if self.cpp11 else 0, threads)
+                                            max_hits, 1 if self.cpp11 else 0, threads)
         return hits, mask
+
+    def _local_hits(self, rays, node_ids, prim_ids):
+        rays = np.ascontiguousarray(rays).reshape(-1)
+        n = len(rays)
+        ids = np.ascontiguousarray(np.broadcast_to(np.asarray(node_ids, np.uint32), (n,)))
+        assert n == 0 or int(ids.max()) < len(self.sg)
+        prims = None if prim_ids is None else np.ascontiguousarray(np.broadcast_to(np.asarray(prim_ids, np.uint32), (n,)))
+        hits, ok = np.zeros(n, SG_HIT_DTYPE), np.zeros(n, np.uint8)
+        self.port.lib.orc_sg_local_hit_batch(_p(self.sg), C.addressof(self._blas_c), _p(rays), n, _p(ids),
+                                             _p(prims) if prims is not None else None, 1 if self.cpp11 else 0,
+                                             _p(hits), _p(ok))
+        return hits, ok.astype(bool)
+
+    def instance_hit(self, rays, node_ids):
+        """(records, ok): the nearest hit of rays[i] inside instance node_ids[i] alone, as Scene::Traverse records
+        it (its per-instance body, nanosg.h:831-850)"""
+        return self._local_hits(rays, node_ids, None)
+
+    def prim_hit(self, rays, node_ids, prim_ids):
+        """(records, ok): the record Scene::Traverse writes when triangle prim_ids[i] of instance node_ids[i] is the
+        pick of rays[i] -- the same arithmetic on that one triangle"""
+        return self._local_hits(rays, node_ids, prim_ids)
 
 
 def list_node_intersections_on_tree(port, nodes, indices, sg_nodes, ray, max_hits=64, cpp11=True):

@@ -52,6 +52,96 @@ def assert_parity(res, allow_ties=True, max_near_ties=None):
         assert res["near_ties"] <= max_near_ties, res
 
 
+def scene_len2(rays):
+    """|d|^2 in float32 in the scene kernel's order, (dx dx + dy dy) + dz dz"""
+    d = rays["dir"].astype(np.float32)
+    return (d[:, 0] * d[:, 0] + d[:, 1] * d[:, 1]) + d[:, 2] * d[:, 2]
+
+
+def scene_handed_over_len(rays):
+    """rays the production scene walk hands to the list kernel for their direction's length: |d|^2 not within
+    1e-5 of 1 (NaN included)"""
+    with np.errstate(invalid="ignore"):
+        return ~(np.abs(scene_len2(rays) - np.float32(1.0)) <= np.float32(1e-5))
+
+
+NEAR_ULPS = 8  # world-distance ulps of a near tie: a few ulps of local t, moved through the transform
+
+
+def _ulp(x):
+    return np.spacing(np.abs(np.float32(x)))
+
+
+def classify_scene_hits(port_scene, rays, got_hits, got_mask, top, top_idx, exact_rays=None):
+    """Production two-level walk vs the oracle's Scene::Traverse over the GPU's own top-level tree (`top`,
+    `top_idx` = Scene.GetTopLevel()), ray by ray.  Asserts:
+      * the same hit mask;
+      * every GPU record is exactly what the reference arithmetic gives for the GPU's (instance, triangle)
+        (PortScene.prim_hit), and its t is the nearest distance inside that instance (PortScene.instance_hit);
+      * where the pick is the oracle's, the whole record is the oracle's;
+      * a different pick is one of three classes:
+        (a) an exact tie, the same bits of t;
+        (b) a distance-versus-entry cull: the reference skips an instance box when the running nearest world
+            DISTANCE is below the box's entry ray PARAMETER tmin, and a hit inside the box can lie below tmin by
+            |1 - |d|| tmin (direction length) plus the rounding of the transform, so the answer depends on the
+            visiting order.  (b) needs the winner's box listed with tmin above the loser's distance (the loser's
+            running nearest can have skipped it) and t_lose - t_win <= |1 - |d|| tmin + NEAR_ULPS ulp;
+        (c) a near tie inside one instance: two triangles of the same instance (coplanar, or meeting at an edge)
+            whose hits lie within NEAR_ULPS ulp; which one the reference reports depends on its visiting order,
+            because its box test culls with the running best t at that precision -- the near tie of compare_hits.
+            The GPU's pick is likewise within NEAR_ULPS ulp of PortScene.instance_hit.
+    `exact_rays` (bool mask): rays that must equal the oracle bit for bit (handed to the list kernel, which runs
+    the reference's own order); a tie is still allowed there when the instance trees are not the oracle's.
+    Returns ({"hits", "same", "ties", "order", "near", "exact_rays"} counts, the oracle's records)."""
+    ph, pm = port_scene.traverse(rays, threads=8, top=top, top_idx=top_idx)
+    got_mask = np.asarray(got_mask).astype(bool)
+    want_mask = pm.astype(bool)
+    bad = np.flatnonzero(got_mask != want_mask)
+    assert len(bad) == 0, f"hit mask differs on {len(bad)} rays, first {bad[:8]}"
+    hit = np.flatnonzero(want_mask)
+    g, w = got_hits[hit], ph[hit]
+    # the GPU's record is the reference arithmetic for its own pick
+    rt, ok = port_scene.prim_hit(rays[hit], g["node_id"], g["prim_id"])
+    assert ok.all() and rt.tobytes() == g.tobytes(), "a GPU record is not prim_hit(node_id, prim_id)"
+    it, ok = port_scene.instance_hit(rays[hit], g["node_id"])
+    assert ok.all()
+    near = np.abs(it["t"].astype(np.float64) - g["t"]) <= NEAR_ULPS * _ulp(it["t"])
+    assert near.all(), f"{int((~near).sum())} GPU picks are not the nearest hit of their instance, first " \
+        f"{hit[~near][:4]}"
+    same = (g["node_id"] == w["node_id"]) & (g["prim_id"] == w["prim_id"])
+    assert g[same].tobytes() == w[same].tobytes()
+    out = {"hits": len(hit), "same": int(same.sum()), "ties": 0, "order": 0, "near": 0, "exact_rays": 0}
+    if exact_rays is not None:
+        ex = np.asarray(exact_rays, bool)[hit]
+        out["exact_rays"] = int(ex.sum())
+    else:
+        ex = np.zeros(len(hit), bool)
+    len2 = scene_len2(rays[hit])
+    unexplained = []
+    for j in np.flatnonzero(~same):
+        tg, tr = np.float32(g["t"][j]), np.float32(w["t"][j])
+        if tg.view(np.uint32) == tr.view(np.uint32):
+            out["ties"] += 1
+            continue
+        if not ex[j]:
+            t_win, t_lose = min(tg, tr), max(tg, tr)
+            win_node = g["node_id"][j] if tg < tr else w["node_id"][j]
+            tmin, _, ids = port_scene.list_node_intersections(rays[hit[j]], top=top, top_idx=top_idx)
+            k = np.flatnonzero(ids == win_node)
+            if len(k):
+                tb = np.float32(tmin[k[0]])
+                slack = abs(1.0 - np.sqrt(np.float64(len2[j]))) * float(tb) + NEAR_ULPS * float(_ulp(t_lose))
+                if t_lose < tb and float(t_lose) - float(t_win) <= slack:
+                    out["order"] += 1
+                    continue
+        if g["node_id"][j] == w["node_id"][j] and abs(float(tg) - float(tr)) <= NEAR_ULPS * float(_ulp(max(tg, tr))):
+            out["near"] += 1
+            continue
+        unexplained.append((int(hit[j]), g[j], w[j]))
+    assert not unexplained, f"{len(unexplained)} picks differ outside the three classes, first: {unexplained[:3]}"
+    return out, ph
+
+
 def check_tree_structure(nodes, indices, verts, faces, min_leaf=4, max_depth=256, preorder=True):
     """Structural invariants every nanort-layout tree must satisfy (SURVEY.md section 4.3, 8b)."""
     n_prims = len(faces)

@@ -4,7 +4,7 @@ tests/test_oracle_scene.py pins bit-for-bit to the unmodified reference):
   * conformance commit: top-level tree bit-equal,
   * conformance traversal: every record bit-equal,
   * fast traversal: same hit mask; records bit-equal where the same (instance, triangle) is picked, and a different
-    pick only at the same world distance,
+    pick only at an exact tie or by a parameter-versus-distance cull (tests/test_gpu_scene_exact.py goes further),
   * the 64-box limit and the flattened-scene cross-check."""
 import numpy as np
 import pytest
@@ -91,6 +91,7 @@ def test_conformance_scene_is_bit_exact(kind):
 
 @pytest.mark.parametrize("kind,top_flags", [("mixed", "fast"), ("row", "fast"), ("mixed", "ref")])
 def test_fast_scene_matches_reference_up_to_equal_distance_ties(kind, top_flags):
+    from helpers import classify_scene_hits, scene_handed_over_len
     from nanort_b200 import api, scenes as S
     from oracle import orc
 
@@ -100,21 +101,11 @@ def test_fast_scene_matches_reference_up_to_equal_distance_ties(kind, top_flags)
     rays = _rays_for(insts, 200000, seed=6)
     if kind == "row":
         rays = _row_rays(rays)
-    ph, pm = port.traverse(rays, threads=8)
     gh, gm = sc.Traverse(rays)
-    assert np.array_equal(pm, gm)
-    hit = pm == 1
-    same_pick = hit & (ph["node_id"] == gh["node_id"]) & (ph["prim_id"] == gh["prim_id"])
-    # same pick -> the whole record is the reference's arithmetic
-    assert _same_bits(ph[same_pick], gh[same_pick])
-    other = hit & ~same_pick
-    # a different pick is legal only at the same world distance (coincident instances / shared edges)
-    assert other.sum() <= (0.05 if kind == "row" else 0.02) * hit.sum()  # row: four coincident instances
-    if other.any():
-        rel = np.abs(ph["t"][other] - gh["t"][other]) / np.maximum(ph["t"][other], 1e-6)
-        assert rel.max() <= 1e-5
-    if kind == "mixed":  # exact ties only (the scaled Cornell box has coincident surfaces)
-        assert other.sum() <= 0.005 * hit.sum()
+    top, ti = sc.GetTopLevel()
+    # a different pick only at an exact tie of t or by a parameter-versus-distance cull (helpers.classify_scene_hits)
+    res, _ = classify_scene_hits(port, rays, gh, gm, top, ti, exact_rays=scene_handed_over_len(rays))
+    assert res["hits"] > 1000, res
 
 
 def test_two_level_equals_flattened_scene():

@@ -376,6 +376,7 @@ def test_scene_with_deep_instances_matches_the_oracle_scene():
     import torch
     from nanort_b200 import api, scenes as S
     from oracle import orc
+    from helpers import classify_scene_hits, scene_handed_over_len
     from test_gpu_scene import _gpu_scene, _rays_for, _same_bits
 
     insts = _deep_scene_instances()
@@ -390,15 +391,10 @@ def test_scene_with_deep_instances_matches_the_oracle_scene():
         ph, pm = port.traverse(rays, threads=8)
         gh, gm = sc.Traverse(rays)
         assert pm.sum() > 2000
-        assert np.array_equal(pm, gm)
+        tn, ti = sc.GetTopLevel()
+        # shared edges of the heightfield: exact ties; otherwise the classes of helpers.classify_scene_hits
+        classify_scene_hits(port, rays, gh, gm, tn, ti, exact_rays=scene_handed_over_len(rays))
         hit = pm == 1
-        same_pick = hit & (ph["node_id"] == gh["node_id"]) & (ph["prim_id"] == gh["prim_id"])
-        assert _same_bits(ph[same_pick], gh[same_pick])
-        other = hit & ~same_pick
-        assert other.sum() <= 0.005 * hit.sum()  # shared edges of the heightfield: equal distances only
-        if other.any():
-            rel = np.abs(ph["t"][other] - gh["t"][other]) / np.maximum(ph["t"][other], 1e-6)
-            assert rel.max() <= 1e-5
         if top == api.BUILD_REFERENCE_TREE:
             ch, cm = sc.Traverse(rays, flags=api.TRAVERSE_CONFORMANCE)
             assert np.array_equal(pm, cm) and _same_bits(ph[hit], ch[cm == 1])

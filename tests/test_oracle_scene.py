@@ -78,6 +78,45 @@ def test_port_scene_matches_reference(kind, cpp11):
     assert _same_bits(rh[hit], ph[hit])
 
 
+@pytest.mark.parametrize("cpp11", [True, False])
+@pytest.mark.parametrize("kind", ["mixed", "row", "hostile"])
+def test_instance_and_prim_hit_reproduce_every_reference_record(kind, cpp11):
+    """PortScene.instance_hit / prim_hit (the per-instance body of Scene::Traverse, on the whole local tree or on one
+    triangle) give back every record of the unmodified nanosg.h bit for bit: the GPU scene tests re-test picks with
+    them."""
+    from edge_cases import hostile_rays
+
+    if not orc.ReferenceScene.available(cpp11):
+        pytest.skip("mode not built")
+    insts = S.instances_row() if kind == "row" else S.instances_mixed(12 if kind == "hostile" else 24)
+    ref = orc.ReferenceScene(insts, cpp11)
+    port = orc.PortScene(insts, cpp11)
+    if kind == "hostile":
+        rays = hostile_rays(np.float32([-8, -4, -8]), np.float32([8, 4, 8]), n=8000, seed=6)
+    else:
+        rays = _scene_rays(insts, 8000, seed=9)
+    rh, rm = ref.traverse(rays, threads=4)
+    hit = np.flatnonzero(rm)
+    assert len(hit) > 300
+    want = rh[hit]
+    for got, ok in (port.prim_hit(rays[hit], want["node_id"], want["prim_id"]),
+                    port.instance_hit(rays[hit], want["node_id"])):
+        assert ok.all() and _same_bits(got, want)
+    # the list cut: max_hits=64 is the reference; a larger cut can only add boxes behind the 64 nearest
+    ph, pm = port.traverse(rays, threads=4, max_hits=64)
+    assert np.array_equal(pm, rm) and _same_bits(ph[hit], want)
+    if kind == "row":
+        k = np.arange(200)
+        rows = rays[:200].copy()
+        rows["org"] = np.stack([-3.0 + 0 * k, 0.3 * S.rand01(k, 0, 4) - 0.15, 0.3 * S.rand01(k, 1, 4) - 0.15], axis=1)
+        rows["dir"] = (1.0, 0.0, 0.0)
+        rows["min_t"], rows["max_t"] = 0.0, 1e30
+        assert all(len(port.list_node_intersections(r, max_hits=128)[0]) > 64 for r in rows)
+        h64, m64 = port.traverse(rows, max_hits=64)
+        h128, m128 = port.traverse(rows, max_hits=128)
+        assert np.array_equal(m64, m128) and _same_bits(h64[m64 == 1], h128[m128 == 1])  # the first sphere wins
+
+
 def test_cull_back_face_flag_is_inert_and_local_ray_is_unbounded():
     """S2 / S4 of the restatement header: the world ray's min_t/max_t gate only the top-level walk."""
     insts = S.instances_mixed(6)
