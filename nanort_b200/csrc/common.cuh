@@ -100,6 +100,22 @@ struct PackedTri {
 };
 static_assert(sizeof(PackedTri) == 48, "PackedTri");
 
+// Rules of the child-pair layouts for either node type (Node40 -> WideNode, layout.cu; Node64 -> PairNodeD,
+// f64_fast.cuh): a branch gets the child-pair record whose index is the exclusive scan of these flags, and a child's
+// reference in its parent's record is that index (branch), kEmptyLeaf (leaf without primitives) or ~first slot (leaf).
+template <class NodeT>
+__global__ void branch_flags_kernel(const NodeT *__restrict__ nodes, uint32_t n, uint32_t *__restrict__ flags) {
+  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) flags[i] = nodes[i].flag == 0 ? 1u : 0u;
+}
+
+template <class NodeT>
+__device__ __forceinline__ int child_ref(const NodeT &c, uint32_t cidx, const uint32_t *widx) {
+  if (c.flag == 0) return (int)widx[cidx];
+  if (c.data[0] == 0) return kEmptyLeaf;
+  return ~(int)c.data[1];
+}
+
 // ---- round-2 traversal layout (traverse_fast3_kernel) ------------------------------------------------------
 // PairNode, 128 bytes = one L1 line, one per BRANCH node, both child boxes.  Every axis owns one 32-byte sector that
 // holds the four planes of that axis in BOTH orders,
@@ -228,7 +244,7 @@ struct DeviceGuard {
   nrt::DeviceGuard _nrt_dg((dev)); \
   NRT_CUDA(_nrt_dg.err)
 
-inline TraceOptions16 default_trace_options() {
+__host__ __device__ inline TraceOptions16 default_trace_options() {
   TraceOptions16 o;
   o.prim_ids_range[0] = 0;
   o.prim_ids_range[1] = 0x7FFFFFFFu;

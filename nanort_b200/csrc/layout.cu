@@ -40,17 +40,6 @@ __global__ void pack_boxes_kernel(const uint32_t *__restrict__ indices, const fl
   out[slot] = t;
 }
 
-__global__ void branch_flags_kernel(const Node40 *__restrict__ nodes, uint32_t n, uint32_t *__restrict__ flags) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) flags[i] = nodes[i].flag == 0 ? 1u : 0u;
-}
-
-__device__ __forceinline__ int child_ref(const Node40 &c, uint32_t cidx, const uint32_t *widx) {
-  if (c.flag == 0) return (int)widx[cidx];
-  if (c.data[0] == 0) return kEmptyLeaf;
-  return ~(int)c.data[1];
-}
-
 __device__ __forceinline__ void invert_box(Node40 &c) {
   for (int k = 0; k < 3; k++) {
     c.bmin[k] = 3.402823466e38f;

@@ -27,30 +27,13 @@ __device__ __forceinline__ WorldRay load_world(const Ray36 *rays, size_t i) {
   return w;
 }
 
-// safemax / safemin of the reference: (a > b) ? a : b, (a < b) ? a : b
-__device__ __forceinline__ float smax(float a, float b) { return (a > b) ? a : b; }
-__device__ __forceinline__ float smin(float a, float b) { return (a < b) ? a : b; }
-
-// NodeBBoxIntersector::Intersect: plain reciprocal direction, no range clamp, no widening
-__device__ __forceinline__ bool raw_box(const WorldRay &w, float rix, float riy, float riz, const float *bmin,
-                                        const float *bmax, float &tmin) {
+// NodeBBoxIntersector::Intersect: plain reciprocal direction, no range clamp, no widening; box = {bmin[3], bmax[3]}.
+// Both distances (NodeHit::t_min / t_max).
+__device__ __forceinline__ bool raw_box(const WorldRay &w, float rix, float riy, float riz, const float *box,
+                                        float &tmin, float &tmax) {
   const bool sx = w.dx < 0.0f, sy = w.dy < 0.0f, sz = w.dz < 0.0f;
-  const float lox = __ldg(bmin + 0), loy = __ldg(bmin + 1), loz = __ldg(bmin + 2);
-  const float hix = __ldg(bmax + 0), hiy = __ldg(bmax + 1), hiz = __ldg(bmax + 2);
-  const float tnx = ((sx ? hix : lox) - w.ox) * rix, tfx = ((sx ? lox : hix) - w.ox) * rix;
-  const float tny = ((sy ? hiy : loy) - w.oy) * riy, tfy = ((sy ? loy : hiy) - w.oy) * riy;
-  const float tnz = ((sz ? hiz : loz) - w.oz) * riz, tfz = ((sz ? loz : hiz) - w.oz) * riz;
-  tmin = smax(tnz, smax(tny, tnx));
-  const float tmax = smin(tfz, smin(tfy, tfx));
-  return tmin <= tmax;
-}
-
-// same test, both distances (NodeHit::t_min / t_max)
-__device__ __forceinline__ bool raw_box_minmax(const WorldRay &w, float rix, float riy, float riz, const float *bmin,
-                                               const float *bmax, float &tmin, float &tmax) {
-  const bool sx = w.dx < 0.0f, sy = w.dy < 0.0f, sz = w.dz < 0.0f;
-  const float lox = __ldg(bmin + 0), loy = __ldg(bmin + 1), loz = __ldg(bmin + 2);
-  const float hix = __ldg(bmax + 0), hiy = __ldg(bmax + 1), hiz = __ldg(bmax + 2);
+  const float lox = __ldg(box + 0), loy = __ldg(box + 1), loz = __ldg(box + 2);
+  const float hix = __ldg(box + 3), hiy = __ldg(box + 4), hiz = __ldg(box + 5);
   const float tnx = ((sx ? hix : lox) - w.ox) * rix, tfx = ((sx ? lox : hix) - w.ox) * rix;
   const float tny = ((sy ? hiy : loy) - w.oy) * riy, tfy = ((sy ? loy : hiy) - w.oy) * riy;
   const float tnz = ((sz ? hiz : loz) - w.oz) * riz, tfz = ((sz ? loz : hiz) - w.oz) * riz;
@@ -106,6 +89,33 @@ struct NodeHitHeap {
     sift_up(hole, vt, vid);
   }
 };
+
+// BVHAccel::ListNodeIntersections (nanort.h:2607-2692): the reference-order walk of a box tree over [min_t, max_t]
+// (hit_t never drops), every box of a visited leaf tested with NodeBBoxIntersector and kept in the
+// at-most-max_k-nearest heap, which is then sorted in place: slots 0 .. heap.n - 1 run nearest first.
+// box_of(id) points at the {bmin[3], bmax[3]} of box primitive id.
+template <class BoxOf>
+__device__ __forceinline__ void collect_node_hits(const Node40 *nodes, const uint32_t *indices, BoxOf box_of,
+                                                  const WorldRay &w, const RayCtx &c, int max_k, NodeHitHeap &heap) {
+  const float rix = 1.0f / w.dx, riy = 1.0f / w.dy, riz = 1.0f / w.dz;  // NodeBBoxIntersector::PrepareTraversal
+  heap.n = 0;
+  reference_walk(nodes, c, w.min_t, w.max_t, [&](uint32_t first, uint32_t count, float &) {
+    for (uint32_t k = 0; k < count; k++) {
+      const uint32_t id = __ldg(indices + first + k);
+      float tmin, tmax;
+      if (!raw_box(w, rix, riy, riz, box_of(id), tmin, tmax)) continue;
+      if (heap.n < max_k) {
+        heap.push(tmin, id);
+      } else if (tmin < heap.t[0]) {
+        heap.pop();
+        heap.push(tmin, id);
+      }
+    }
+  });
+  const int n_hits = heap.n;
+  for (int k = 0; k < n_hits; k++) heap.pop();  // in-place heap sort
+  heap.n = n_hits;
+}
 
 
 }  // namespace nrt

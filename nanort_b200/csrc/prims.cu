@@ -194,52 +194,17 @@ __global__ void __launch_bounds__(128)
   const WorldRay w = load_world(rays, i);
   RayCtx c;
   setup_ray(c, w.ox, w.oy, w.oz, w.dx, w.dy, w.dz, w.min_t, (flags & NRT_TRAVERSE_CPP03_INVERSE) != 0);
-  const float rix = 1.0f / w.dx, riy = 1.0f / w.dy, riz = 1.0f / w.dz;  // NodeBBoxIntersector::PrepareTraversal
   NodeHitHeap heap;
-  heap.n = 0;
-  float tmaxs[kMaxNodeHits + 1];  // t_max of the entry with the same id is looked up again at the end (cheap: K <= 64)
-  (void)tmaxs;
-  uint32_t stack[kPrimStack];
-  int sp = range_has_nan(w.min_t, w.max_t) ? -1 : 0;
-  stack[0] = 0;
-  while (sp >= 0) {
-    const Node40 *nd = nodes + stack[sp];
-    sp--;
-    const float *f = reinterpret_cast<const float *>(nd);
-    float tn;
-    if (!slab(c, __ldg(f + 0), __ldg(f + 1), __ldg(f + 2), __ldg(f + 3), __ldg(f + 4), __ldg(f + 5), w.min_t, w.max_t, tn))
-      continue;
-    const uint32_t d0 = __ldg(&nd->data[0]), d1 = __ldg(&nd->data[1]);
-    if (__ldg(&nd->flag) == 0) {
-      const int axis = __ldg(&nd->axis);
-      const int sgn = axis == 0 ? c.sx : (axis == 1 ? c.sy : c.sz);
-      if (sp + 2 < kPrimStack) {
-        stack[++sp] = sgn ? d0 : d1;
-        stack[++sp] = sgn ? d1 : d0;
-      }
-      continue;
-    }
-    for (uint32_t k = 0; k < d0; k++) {
-      const uint32_t id = __ldg(indices + d1 + k);
-      float tmin;
-      if (!raw_box(w, rix, riy, riz, boxes6 + 6 * (size_t)id, boxes6 + 6 * (size_t)id + 3, tmin)) continue;
-      if (heap.n < max_k) {
-        heap.push(tmin, id);
-      } else if (tmin < heap.t[0]) {
-        heap.pop();
-        heap.push(tmin, id);
-      }
-    }
-  }
-  const int n_hits = heap.n;
-  for (int k = 0; k < n_hits; k++) heap.pop();  // in-place heap sort: slots 0..n_hits-1 now run nearest first
-  for (int k = 0; k < n_hits; k++) {
+  collect_node_hits(nodes, indices, [=](uint32_t id) { return boxes6 + 6 * (size_t)id; }, w, c, max_k, heap);
+  // t_max of each listed box, recomputed (cheap: K <= 64)
+  const float rix = 1.0f / w.dx, riy = 1.0f / w.dy, riz = 1.0f / w.dz;
+  for (int k = 0; k < heap.n; k++) {
     const uint32_t id = heap.id[k];
     float tmin, tmax;
-    raw_box_minmax(w, rix, riy, riz, boxes6 + 6 * (size_t)id, boxes6 + 6 * (size_t)id + 3, tmin, tmax);
+    raw_box(w, rix, riy, riz, boxes6 + 6 * (size_t)id, tmin, tmax);
     out_hits[i * (size_t)max_k + k] = NodeHit12{heap.t[k], tmax, id};
   }
-  out_count[i] = (uint32_t)n_hits;
+  out_count[i] = (uint32_t)heap.n;
 }
 
 }  // namespace
