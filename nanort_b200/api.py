@@ -449,16 +449,21 @@ class BVHAccel:
                                             C.c_void_p(stream) if stream else None))
         return res
 
-    def BuildSpheres(self, centers, radii, options=None):
+    def BuildSpheres(self, centers, radii, options=None, center_stride_bytes=12):
         """BVHAccel::Build(n, SphereGeometry(centers, radii), SpherePred(centers), options) of the reference's
-        particle_primitive model (nrt_build_prims, NRT_PRIM_SPHERES).  Traverse() then returns sphere hit records."""
+        particle_primitive model (nrt_build_prims, NRT_PRIM_SPHERES).  Traverse() then returns sphere hit records.
+        Centre i is the three floats at byte offset i * center_stride_bytes of `centers` (a multiple of 4, >= 12).
+        Traverse flags on the result: TRAVERSE_CPP03_INVERSE as for triangles; TRAVERSE_CONFORMANCE and TRAVERSE_ANY_HIT
+        are ignored (closest hit, the same records); TRAVERSE_RAY32, CountDevice and LaneStatsDevice are refused."""
         self.free()
         self._set_device()
-        centers = np.ascontiguousarray(centers, np.float32).reshape(-1, 3)
         radii = np.ascontiguousarray(radii, np.float32)
-        assert len(radii) == len(centers)
+        centers = np.ascontiguousarray(centers, np.float32).reshape(-1)
+        assert center_stride_bytes >= 12 and center_stride_bytes % 4 == 0
+        assert len(radii) == 0 or centers.size * 4 >= (len(radii) - 1) * center_stride_bytes + 12
         h = C.c_void_p()
-        rc = lib().nrt_build_prims(PRIM_SPHERES, _p(centers), 12, _p(radii), len(radii), _p(options), C.byref(h))
+        rc = lib().nrt_build_prims(PRIM_SPHERES, _p(centers), int(center_stride_bytes), _p(radii), len(radii), _p(options),
+                                   C.byref(h))
         if rc != 0:
             if len(radii) == 0:
                 return False

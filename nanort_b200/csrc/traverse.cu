@@ -333,6 +333,10 @@ int launch_traverse_path_shadow(const Accel *a, const PathQueues &q, const unsig
 
 int launch_traverse_count(const Accel *a, const Ray36 *d_rays, size_t n, const TraceOptions16 &opt,
                           uint32_t flags, uint64_t *d_counts2, cudaStream_t s) {
+  if (a->prim_kind != 0) {  // both counting walks test triangles: their counts would mean nothing on other kinds
+    set_error("nrt_traverse_count_device / nrt_traverse_lane_stats_device: counting walks need a triangle accel");
+    return NRT_ERR_INVALID;
+  }
   NRT_CUDA(cudaMemsetAsync(d_counts2, 0, 16 * sizeof(uint64_t), s));  // [0] boxes, [1] prims, [2..15] lane statistics
   if (n == 0) return NRT_OK;
   AosRays r{d_rays};

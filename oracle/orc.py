@@ -703,25 +703,98 @@ class ReferencePathTracer:
 
 
 class ReferenceSpheres:
-    """The reference's custom-primitive model (oracle/_ref/libprim_ref.so = the unmodified
-    examples/particle_primitive/main.cc: SphereGeometry, SpherePred, SphereIntersector) on the unmodified BVHAccel."""
+    """The reference's custom-primitive model (oracle/_ref/libprim_ref{,03}.so = the unmodified
+    examples/particle_primitive/main.cc: SphereGeometry, SpherePred, SphereIntersector) on the unmodified BVHAccel.
+    `cpp11=False` is the same model built without NANORT_USE_CPP11_FEATURE (the C++03 vsafe_inverse).  The accel is
+    the reference's own build (`options`: a BUILD_OPT_DTYPE record, None = the defaults) or, through `adopt`, any
+    (nodes, indices) pair -- e.g. the device's tree -- loaded with the reference's own Load."""
+
+    _libs = {}
 
     @staticmethod
-    def available():
-        return os.path.exists(os.path.join(HERE, "_ref", "libprim_ref.so"))
+    def _name(cpp11):
+        return "libprim_ref.so" if cpp11 else "libprim_ref03.so"
 
-    def __init__(self, centers, radii):
-        L = C.CDLL(os.path.join(HERE, "_ref", "libprim_ref.so"))
-        L.refsph_build.restype = C.c_void_p
-        L.refsph_build.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
-        L.refsph_free.argtypes = [C.c_void_p]
-        L.refsph_bounding_box.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-        L.refsph_traverse.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_int]
-        self.L = L
+    # the entry points added after the first version of the shim (refsph_build / refsph_traverse / refsph_free /
+    # refsph_bounding_box): an oracle/_ref built from that version has none of them
+    _EXACT = ("refsph_mode_cpp11", "refsph_build_opts", "refsph_adopt", "refsph_traverse_opts", "refsph_test_prims",
+              "refsph_nan_rays", "refsph_node_box_hit")
+
+    @staticmethod
+    def available(cpp11=True):
+        """the library exists: Build with the default options and Traverse with a prim id range"""
+        return os.path.exists(os.path.join(HERE, "_ref", ReferenceSpheres._name(cpp11)))
+
+    @classmethod
+    def exact_available(cls, cpp11=True):
+        """the library also has adopt, build and trace options, test_prim, nan_rays and box_hit"""
+        if not cls.available(cpp11):
+            return False
+        L = cls._lib(cpp11)
+        return all(hasattr(L, f) for f in cls._EXACT)
+
+    @classmethod
+    def _lib(cls, cpp11):
+        if cpp11 in cls._libs:
+            return cls._libs[cpp11]
+        L = C.CDLL(os.path.join(HERE, "_ref", cls._name(cpp11)))
+        vp, sz = C.c_void_p, C.c_size_t
+        L.refsph_build.restype = vp
+        L.refsph_build.argtypes = [vp, vp, sz]
+        L.refsph_free.argtypes = [vp]
+        L.refsph_bounding_box.argtypes = [vp, vp, vp]
+        L.refsph_traverse.argtypes = [vp, vp, sz, vp, vp, C.c_uint32, C.c_uint32, C.c_int]
+        if all(hasattr(L, f) for f in cls._EXACT):
+            L.refsph_mode_cpp11.restype = C.c_int
+            L.refsph_build_opts.restype = vp
+            L.refsph_build_opts.argtypes = [vp, vp, sz, vp]
+            L.refsph_adopt.restype = vp
+            L.refsph_adopt.argtypes = [vp, sz, vp, sz, vp, vp, sz]
+            L.refsph_num_nodes.restype = sz
+            L.refsph_num_nodes.argtypes = [vp]
+            L.refsph_num_indices.restype = sz
+            L.refsph_num_indices.argtypes = [vp]
+            L.refsph_copy_nodes.argtypes = [vp, vp]
+            L.refsph_copy_indices.argtypes = [vp, vp]
+            L.refsph_traverse_opts.argtypes = [vp, vp, sz, vp, vp, vp, C.c_int]
+            L.refsph_test_prims.argtypes = [vp, vp, sz, vp, vp, vp, vp, vp]
+            L.refsph_nan_rays.argtypes = [vp, vp, sz, vp, vp, C.c_int]
+            L.refsph_node_box_hit.restype = C.c_int
+            L.refsph_node_box_hit.argtypes = [vp, vp, sz]
+            assert L.refsph_mode_cpp11() == (1 if cpp11 else 0)
+        cls._libs[cpp11] = L
+        return L
+
+    def _need_exact(self, what):
+        if not all(hasattr(self.L, f) for f in self._EXACT):
+            raise RuntimeError(f"ReferenceSpheres.{what} needs an oracle/_ref built from the current prim_ref_shim.cc "
+                               "(ReferenceSpheres.exact_available())")
+
+    def __init__(self, centers, radii, cpp11=True, options=None, _adopt=None):
+        self.L = L = self._lib(cpp11)
+        self.cpp11 = cpp11
         self.centers = np.ascontiguousarray(centers, np.float32).reshape(-1, 3)
         self.radii = np.ascontiguousarray(radii, np.float32)
-        self.h = L.refsph_build(_p(self.centers), _p(self.radii), len(self.radii))
-        assert self.h, "reference Build returned false"
+        assert len(self.centers) == len(self.radii)
+        if _adopt is None and options is None:
+            self.h = L.refsph_build(_p(self.centers), _p(self.radii), len(self.radii))
+            assert self.h, "reference Build returned false"
+        elif _adopt is None:
+            self._need_exact("options")
+            self.h = L.refsph_build_opts(_p(self.centers), _p(self.radii), len(self.radii), _p(options))
+            assert self.h, "reference Build returned false"
+        else:
+            self._need_exact("adopt")
+            nodes, indices = np.ascontiguousarray(_adopt[0]), np.ascontiguousarray(_adopt[1], np.uint32)
+            assert nodes.dtype.itemsize == 40
+            self.h = L.refsph_adopt(_p(nodes), len(nodes), _p(indices), len(indices), _p(self.centers), _p(self.radii),
+                                    len(self.radii))
+            assert self.h, "reference Load returned false"
+
+    @classmethod
+    def adopt(cls, nodes, indices, centers, radii, cpp11=True):
+        """The reference's Traverse and SphereIntersector over a given tree (BVHAccel::Load of its Dump format)."""
+        return cls(centers, radii, cpp11=cpp11, _adopt=(nodes, indices))
 
     def __del__(self):
         if getattr(self, "h", None):
@@ -733,9 +806,83 @@ class ReferenceSpheres:
         self.L.refsph_bounding_box(self.h, _p(a), _p(b))
         return a, b
 
-    def traverse(self, rays, prim_range=(0, 0x7FFFFFFF), threads=8):
+    def nodes(self):
+        self._need_exact("nodes")
+        out = np.zeros(self.L.refsph_num_nodes(self.h), NODE_DTYPE)
+        self.L.refsph_copy_nodes(self.h, _p(out))
+        return out
+
+    def indices(self):
+        self._need_exact("indices")
+        out = np.zeros(self.L.refsph_num_indices(self.h), np.uint32)
+        self.L.refsph_copy_indices(self.h, _p(out))
+        return out
+
+    @staticmethod
+    def _topts(prim_range, topts):
+        if topts is None:
+            topts = trace_options()
+            if prim_range is not None:
+                topts["prim_ids_range"] = prim_range
+        else:
+            assert prim_range is None
+        return np.ascontiguousarray(topts, TRACE_OPT_DTYPE)
+
+    def traverse(self, rays, prim_range=None, threads=8, topts=None):
+        """One Traverse per ray: (hits, mask); hits are zero on a miss.  topts: a TRACE_OPT_DTYPE record, passed whole."""
         rays = np.ascontiguousarray(rays)
+        assert rays.dtype.itemsize == 36
         hits = np.zeros(len(rays), HIT_DTYPE)
         mask = np.zeros(len(rays), np.uint8)
-        self.L.refsph_traverse(self.h, _p(rays), len(rays), _p(hits), _p(mask), int(prim_range[0]), int(prim_range[1]), int(threads))
+        t = self._topts(prim_range, topts)
+        if hasattr(self.L, "refsph_traverse_opts"):
+            self.L.refsph_traverse_opts(self.h, _p(rays), len(rays), _p(hits), _p(mask), _p(t), int(threads))
+        else:  # the first version of the shim: the default trace options with an id range
+            d = trace_options()
+            assert all(int(d[f][0]) == int(t[f][0]) for f in ("skip_prim_id", "cull_back_face")), \
+                "trace options other than prim_ids_range need ReferenceSpheres.exact_available()"
+            lo, hi = (int(x) for x in t["prim_ids_range"][0])
+            self.L.refsph_traverse(self.h, _p(rays), len(rays), _p(hits), _p(mask), lo, hi, int(threads))
         return hits, mask
+
+    def test_prim(self, rays, prims, t_inout=None, prim_range=None, topts=None):
+        """SphereIntersector::Intersect of sphere prims[i] on rays[i] from t = t_inout[i] (None: ray.max_t), then
+        PostTraversal: (records, ok) -- the reference's full record had its Traverse picked prims[i]; ok = Intersect's
+        return value (records are zero where it is False)."""
+        self._need_exact("test_prim")
+        rays = np.ascontiguousarray(rays).reshape(-1)
+        prims = np.ascontiguousarray(np.broadcast_to(np.asarray(prims, np.uint32), (len(rays),)))
+        if t_inout is not None:
+            t_inout = np.ascontiguousarray(np.broadcast_to(np.asarray(t_inout, np.float32), (len(rays),)))
+        hits = np.zeros(len(rays), HIT_DTYPE)
+        ok = np.zeros(len(rays), np.uint8)
+        self.L.refsph_test_prims(self.h, _p(rays), len(rays), _p(prims), _p(t_inout) if t_inout is not None else None,
+                                 _p(self._topts(prim_range, topts)), _p(hits), _p(ok))
+        return hits, ok.astype(bool)
+
+    def nan_rays(self, rays, prim_range=None, topts=None, threads=8):
+        """Rays for which some sphere inside the id range yields a NaN t (brute force over all spheres)."""
+        self._need_exact("nan_rays")
+        rays = np.ascontiguousarray(rays)
+        out = np.zeros(len(rays), np.uint8)
+        self.L.refsph_nan_rays(self.h, _p(rays), len(rays), _p(self._topts(prim_range, topts)), _p(out), int(threads))
+        return out.astype(bool)
+
+    def leaf_of(self):
+        """leaf node index of every sphere in this accel's tree"""
+        nodes, idx = self.nodes(), self.indices()
+        leaves = np.flatnonzero(nodes["flag"] == 1)
+        cnt, off = nodes["data"][leaves, 0].astype(np.int64), nodes["data"][leaves, 1].astype(np.int64)
+        start = np.cumsum(cnt) - cnt
+        slot = np.repeat(off, cnt) + (np.arange(int(cnt.sum())) - np.repeat(start, cnt))
+        out = np.full(len(self.radii), -1, np.int64)
+        out[idx[slot]] = np.repeat(leaves, cnt)
+        return out
+
+    def box_hit(self, ray, node):
+        """Whether the box of `node` passes the reference's slab test over [ray.min_t, ray.max_t]."""
+        self._need_exact("box_hit")
+        ray = np.ascontiguousarray(ray).reshape(1)
+        r = self.L.refsph_node_box_hit(self.h, _p(ray), int(node))
+        assert r >= 0, f"no node {node}"
+        return bool(r)

@@ -97,6 +97,7 @@ def test_list_node_intersections_matches_the_reference(max_hits):
     restatement, itself pinned to the unmodified nanosg.h on the reference's tree -- re-checked below), and with the
     reference's own list on every ray whose answer cannot depend on the leaves (all listed boxes start in front of
     min_t)."""
+    from edge_cases import hostile_rays
     from oracle import orc
     from nanort_b200 import api, scenes as S
 
@@ -145,3 +146,35 @@ def test_list_node_intersections_matches_the_reference(max_hits):
             tree_independent += 1
         many += int(counts[i] >= min(max_hits, 10))
     assert many > 20 and tree_independent > 100
+    # the C++03 inverse (-0.0 -> +inf) and the hostile rays of tests/edge_cases.py (NaN / inf / zero components,
+    # inverted and NaN ranges), against the restatement on the device's tree in each convention; the restatement's
+    # C++03 convention is pinned to the unmodified nanosg.h built without NANORT_USE_CPP11_FEATURE on its own tree
+    hostile = hostile_rays(bmin - 1, bmax + 1, 1200, seed=6)
+    both = np.concatenate([rays, hostile])
+    for cpp11 in (True, False):
+        flags = 0 if cpp11 else api.TRAVERSE_CPP03_INVERSE
+        hits, counts = acc.ListNodeIntersections(both, max_intersections=max_hits, flags=flags)
+        for i in range(len(rays) if cpp11 else 0, len(both)):
+            tmin, tmax, ids = orc.list_node_intersections_on_tree(port, dev_nodes, dev_idx, st, both[i], max_hits,
+                                                                  cpp11=cpp11)
+            assert counts[i] == len(ids), (cpp11, i, counts[i], len(ids))
+            g = hits[i, : counts[i]]
+            assert np.array_equal(g["node_id"], ids), (cpp11, i)
+            assert _same_f32(g["t_min"], tmin) and _same_f32(g["t_max"], tmax), (cpp11, i)
+    if orc.ReferenceScene.available(False):
+        ref03 = orc.ReferenceScene(insts, cpp11=False)
+        n03, i03 = ref03.top()
+        st03 = ref03.node_states()
+        for i in range(len(rays), len(both), 3):
+            r_tmin, r_tmax, r_ids = ref03.list_node_intersections(both[i], max_hits)
+            o_tmin, o_tmax, o_ids = orc.list_node_intersections_on_tree(port, n03, i03, st03, both[i], max_hits, cpp11=False)
+            assert np.array_equal(o_ids, r_ids) and _same_f32(o_tmin, r_tmin), i
+
+
+def _same_f32(a, b):
+    """bit for bit, except that any NaN equals any NaN (the device and the host spell NaN differently)"""
+    a, b = np.asarray(a, np.float32), np.asarray(b, np.float32)
+    if a.shape != b.shape:
+        return False
+    both_nan = np.isnan(a) & np.isnan(b)
+    return bool(np.all(both_nan | (a.view(np.uint32) == b.view(np.uint32))))
