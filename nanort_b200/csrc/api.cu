@@ -49,6 +49,10 @@ static void destroy(Accel *a) {
   cudaFree(a->d_tris);
   cudaFree(a->d_pair);
   cudaFree(a->d_tris_cm);
+  cudaFree(a->d_pair_rel);
+  cudaFree(a->d_tris_rel);
+  cudaFree(a->d_face_n);
+  if (a->ao_pass_done) cudaEventDestroy(a->ao_pass_done);
   cudaFree(a->d_prim_boxes);
   cudaFree(a->d_prim_data);
   cudaFree(a->d_wave);

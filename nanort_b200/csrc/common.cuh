@@ -162,6 +162,17 @@ struct Accel {
   PackedTri *d_tris = nullptr;
   PairNode *d_pair = nullptr;  // same indices and refs as d_wide
   TriCM *d_tris_cm = nullptr;  // same slots as d_tris
+  // camera-relative copies of d_pair / d_tris_cm (every plane and vertex minus the camera origin rel_origin, bit
+  // patterns of three floats), read by the AO pass's camera launch; derived on the pass's stream when the origin changes
+  PairNode *d_pair_rel = nullptr;
+  TriCM *d_tris_rel = nullptr;
+  bool rel_valid = false;
+  uint32_t rel_origin[3] = {0, 0, 0};
+  // unit geometric normal per primitive (float4, w unused), read by the AO spawn; derived on the first AO pass
+  float4 *d_face_n = nullptr;
+  // recorded after the last launch of every AO pass; the next pass waits on it (any stream), so that the pass scratch
+  // (d_wave, d_counters[2..6]) and the camera-relative copies are never rewritten while a pass still reads them
+  cudaEvent_t ao_pass_done = nullptr;
   // host mirrors (lazy)
   std::vector<Node40> h_nodes;
   std::vector<uint32_t> h_indices;
@@ -280,6 +291,9 @@ int launch_traverse_soa(const Accel *a, const float4 *d_org_tmin, const float4 *
                         Hit16 *d_hits, const TraceOptions16 &opt, uint32_t flags, cudaStream_t s);
 // layout.cu
 int derive_private_layout(Accel *a, cudaStream_t s);
+// (re)derives d_pair_rel / d_tris_rel on `s` unless they already hold this origin; the caller orders `s` after every
+// launch that may still read the previous copies
+int camera_relative_layout(Accel *a, const float cam[3], cudaStream_t s);
 // build.cu
 int build_on_device(Accel *a, cudaStream_t s);
 // build_ref.cu: the reference-exact builder of BVHAccel<T>, T = float or double.  Inputs on the device: packed T

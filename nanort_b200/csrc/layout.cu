@@ -6,6 +6,10 @@
 //   faces / verts as TriangleMesh holds them (nanort.h:925-930)
 // The packed triangles remove the reference's two levels of indirection at
 // intersection time (indices_ -> faces -> vertices, nanort.h:2394 + 1065-1071).
+#include <string.h>
+
+#include <algorithm>
+
 #include "common.cuh"
 #include "scan.cuh"
 
@@ -117,6 +121,48 @@ __global__ void tris_cm_kernel(const PackedTri *__restrict__ in, uint32_t n, Tri
   out[i] = o;
 }
 
+// Camera-relative copies: every plane and vertex coordinate minus the camera origin's component on its axis (refs,
+// pad and the w words unchanged).  One IEEE subtraction gives the same bits here as in the traversal kernel, which
+// subtracts the origin per ray otherwise (no contraction under --fmad=false), so every decision stays the same.
+__global__ void camera_relative_kernel(const PairNode *__restrict__ pair, uint32_t n_pair, const TriCM *__restrict__ tris,
+                                       uint32_t n_tris, float cx, float cy, float cz, PairNode *__restrict__ pair_rel,
+                                       TriCM *__restrict__ tris_rel) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n_pair) {
+    PairNode p = pair[i];
+    for (int k = 0; k < 2; k++) {
+      p.x[k] = make_float4(p.x[k].x - cx, p.x[k].y - cx, p.x[k].z - cx, p.x[k].w - cx);
+      p.y[k] = make_float4(p.y[k].x - cy, p.y[k].y - cy, p.y[k].z - cy, p.y[k].w - cy);
+      p.z[k] = make_float4(p.z[k].x - cz, p.z[k].y - cz, p.z[k].z - cz, p.z[k].w - cz);
+    }
+    pair_rel[i] = p;
+  }
+  if (i < n_tris) {
+    TriCM t = tris[i];
+    t.X = make_float4(t.X.x - cx, t.X.y - cx, t.X.z - cx, t.X.w);
+    t.Y = make_float4(t.Y.x - cy, t.Y.y - cy, t.Y.z - cy, t.Y.w);
+    t.Z = make_float4(t.Z.x - cz, t.Z.y - cz, t.Z.z - cz, t.Z.w);
+    tris_rel[i] = t;
+  }
+}
+
+int camera_relative_layout(Accel *a, const float cam[3], cudaStream_t s) {
+  uint32_t key[3];
+  memcpy(key, cam, sizeof(key));  // bit patterns: -0.0 and +0.0 give different copies, NaN is a key like any other
+  if (a->rel_valid && key[0] == a->rel_origin[0] && key[1] == a->rel_origin[1] && key[2] == a->rel_origin[2])
+    return NRT_OK;
+  a->rel_valid = false;
+  if (!a->d_pair_rel) NRT_CUDA(cudaMalloc(&a->d_pair_rel, sizeof(PairNode) * a->n_wide));
+  if (!a->d_tris_rel) NRT_CUDA(cudaMalloc(&a->d_tris_rel, sizeof(TriCM) * (size_t)a->n_prims));
+  const uint32_t n = (uint32_t)std::max<size_t>(a->n_wide, a->n_prims);
+  camera_relative_kernel<<<(n + 255) / 256, 256, 0, s>>>(a->d_pair, (uint32_t)a->n_wide, a->d_tris_cm, a->n_prims, cam[0],
+                                                         cam[1], cam[2], a->d_pair_rel, a->d_tris_rel);
+  NRT_CUDA(cudaGetLastError());
+  memcpy(a->rel_origin, key, sizeof(key));
+  a->rel_valid = true;
+  return NRT_OK;
+}
+
 int derive_private_layout(Accel *a, cudaStream_t s) {
   const uint32_t n_nodes = (uint32_t)a->n_nodes;
   const uint32_t n_prims = a->n_prims;
@@ -124,10 +170,17 @@ int derive_private_layout(Accel *a, cudaStream_t s) {
   cudaFree(a->d_wide);
   cudaFree(a->d_pair);
   cudaFree(a->d_tris_cm);
+  cudaFree(a->d_pair_rel);
+  cudaFree(a->d_tris_rel);
+  cudaFree(a->d_face_n);
   a->d_tris = nullptr;
   a->d_wide = nullptr;
   a->d_pair = nullptr;
   a->d_tris_cm = nullptr;
+  a->d_pair_rel = nullptr;
+  a->d_tris_rel = nullptr;
+  a->rel_valid = false;
+  a->d_face_n = nullptr;
   NRT_CUDA(cudaMalloc(&a->d_tris, sizeof(PackedTri) * (size_t)n_prims));
   if (a->d_prim_boxes)
     pack_boxes_kernel<<<(n_prims + 255) / 256, 256, 0, s>>>(a->d_indices, a->d_prim_boxes, n_prims, a->d_tris);

@@ -49,7 +49,7 @@ __global__ void __launch_bounds__(256)
 // one AO ray per primary hit, compacted with one atomic per warp; primary misses count as unoccluded.
 __global__ void __launch_bounds__(256)
     gen_ao_kernel(nrt_ao_params p, unsigned long long slot0, uint32_t count, Wave w,
-                  const float *__restrict__ verts, const uint32_t *__restrict__ faces, float *__restrict__ accum,
+                  const float4 *__restrict__ face_n, float *__restrict__ accum,
                   unsigned long long *counters /* [0] ao rays of this wave */) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   const int lane = threadIdx.x & 31;
@@ -63,7 +63,7 @@ __global__ void __launch_bounds__(256)
       if (h.prim_id == 0xFFFFFFFFu) {
         atomicAdd(accum + pix, 1.0f);
       } else {
-        make_ao_ray(p, pix, slot_sample(p, slot0 + i), w.org_tmin[i], w.dir_tmax[i], h.t, h.prim_id, verts, faces, o4, d4);
+        make_ao_ray(p, pix, slot_sample(p, slot0 + i), w.org_tmin[i], w.dir_tmax[i], h.t, h.prim_id, face_n, o4, d4);
         make = true;
       }
     }
@@ -79,6 +79,17 @@ __global__ void __launch_bounds__(256)
     w.ao_dir_tmax[j] = d4;
     w.ao_pix[j] = pix;
   }
+}
+
+// Accel::d_face_n: the unit normal make_ao_ray() reads, once per primitive instead of once per primary hit
+__global__ void __launch_bounds__(256)
+    face_normals_kernel(const float *__restrict__ verts, const uint32_t *__restrict__ faces, uint32_t n,
+                        float4 *__restrict__ out) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  float nx, ny, nz, a2;
+  geometric_normal(verts, faces, i, nx, ny, nz, a2);
+  out[i] = make_float4(nx, ny, nz, 0.0f);
 }
 
 __global__ void __launch_bounds__(256)
@@ -132,8 +143,8 @@ __global__ void __launch_bounds__(256)
 int launch_traverse_soa_devcount(const Accel *a, const float4 *d_org_tmin, const float4 *d_dir_tmax,
                                  const unsigned long long *d_count, size_t capacity, Hit16 *d_hits,
                                  const TraceOptions16 &opt, uint32_t flags, cudaStream_t s);
-int launch_traverse_camera_fused(const Accel *a, const Wave &w, const nrt_ao_params &p, unsigned long long slot0,
-                                 size_t count, float *d_accum, unsigned long long *d_wave_counters,
+int launch_traverse_camera_fused(Accel *a, const Wave &w, const nrt_ao_params &p, unsigned long long slot0, size_t count,
+                                 const float4 *d_face_n, float *d_accum, unsigned long long *d_wave_counters,
                                  const TraceOptions16 &opt, uint32_t flags, cudaStream_t s);
 int launch_traverse_ao_fused(const Accel *a, const Wave &w, const unsigned long long *d_count, size_t capacity,
                              float *d_accum, unsigned long long *d_totals, const TraceOptions16 &opt, uint32_t flags,
@@ -175,11 +186,31 @@ static int run_ao_pass(const nrt_accel *h, const nrt_ao_params *pp, float *d_acc
     set_error("nrt_render_ao_device: bad parameters (tiles must be multiples of 8x4 pixels)");
     return NRT_ERR_INVALID;
   }
+  // before anything is derived or launched: the face normals and the camera-relative copies are built from the
+  // triangle layout, which sphere / box accels (and the top level of a scene) do not have
+  if (!a->d_pair || !a->d_tris_cm || !a->d_faces) {
+    set_error("nrt_render_ao_device: the AO pass needs a triangle accel");
+    return NRT_ERR_INVALID;
+  }
   NRT_DEVICE(a->device);
   // d_wave and d_counters[2..6] are per-accel scratch: concurrent passes on ONE accel are serialised (passes on
   // different accels, e.g. one per GPU, run concurrently)
   std::lock_guard<std::mutex> lock(a->host_mu);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
+  // host_mu orders the enqueueing only: the previous pass on this accel may still run on another stream, and nothing
+  // it reads (the wave scratch, the counters, the camera-relative copies) is rewritten before it has finished
+  if (!a->ao_pass_done) NRT_CUDA(cudaEventCreateWithFlags(&a->ao_pass_done, cudaEventDisableTiming));
+  NRT_CUDA(cudaStreamWaitEvent(s, a->ao_pass_done, 0));
+  struct RecordOnExit {
+    cudaEvent_t e;
+    cudaStream_t s;
+    ~RecordOnExit() { cudaEventRecord(e, s); }
+  } pass_done{a->ao_pass_done, s};
+  if (!a->d_face_n) {
+    NRT_CUDA(cudaMalloc(&a->d_face_n, sizeof(float4) * (size_t)a->n_prims));
+    face_normals_kernel<<<(a->n_prims + 255) / 256, 256, 0, s>>>(a->d_verts, a->d_faces, a->n_prims, a->d_face_n);
+    NRT_CUDA(cudaGetLastError());
+  }
   const uint32_t tiles_x = (p.width + p.tile_w - 1) / p.tile_w, tiles_y = (p.height + p.tile_h - 1) / p.tile_h;
   const uint32_t n_tiles = tiles_x * tiles_y;
   const uint32_t my_tiles = n_tiles > p.shard ? (n_tiles - p.shard + p.n_shards - 1) / p.n_shards : 0;
@@ -271,7 +302,7 @@ static int run_ao_pass(const nrt_accel *h, const nrt_ao_params *pp, float *d_acc
       // two traversal launches per wave and nothing else: camera rays are generated at ray fetch, the retire
       // steps spawn the AO rays and accumulate visibility
       if (res) cudaEventRecord(t0, s);
-      rc = launch_traverse_camera_fused(a, w, p, s0, count, d_accum, wave_ctr, opt, trav_flags, s);
+      rc = launch_traverse_camera_fused(a, w, p, s0, count, a->d_face_n, d_accum, wave_ctr, opt, trav_flags, s);
       if (rc != NRT_OK) break;
       if (res) {
         cudaEventRecord(t1, s);
@@ -295,7 +326,7 @@ static int run_ao_pass(const nrt_accel *h, const nrt_ao_params *pp, float *d_acc
       if (res) cudaEventRecord(t1, s);
       launches++;
       trav_launches++;
-      gen_ao_kernel<<<grid, 256, 0, s>>>(p, s0, count, w, a->d_verts, a->d_faces, d_accum, wave_ctr);
+      gen_ao_kernel<<<grid, 256, 0, s>>>(p, s0, count, w, a->d_face_n, d_accum, wave_ctr);
       launches++;
       if (dump_ao) {
         unsigned long long n_wave = 0;

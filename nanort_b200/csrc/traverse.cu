@@ -23,6 +23,7 @@ namespace nrt {
 // ------------------------------------------------------------------ ray loaders
 struct AosRays {
   static constexpr int kPayloadWords = 0;
+  static constexpr bool kSharedOrigin = false;  // rays start anywhere (wavefront.cuh, CameraRaysT)
   const Ray36 *rays;
   __device__ __forceinline__ void load(size_t i, float &ox, float &oy, float &oz, float &dx, float &dy,
                                        float &dz, float &tmin, float &tmax, uint32_t * = nullptr) const {
@@ -41,6 +42,7 @@ struct AosRays {
 // 32-byte ray records (NRT_TRAVERSE_RAY32): {org.xyz, dir.x} {dir.yz, min_t, max_t}, two 128-bit loads
 struct Aos32Rays {
   static constexpr int kPayloadWords = 0;
+  static constexpr bool kSharedOrigin = false;  // rays start anywhere (wavefront.cuh, CameraRaysT)
   const float4 *rays;
   __device__ __forceinline__ void load(size_t i, float &ox, float &oy, float &oz, float &dx, float &dy,
                                        float &dz, float &tmin, float &tmax, uint32_t * = nullptr) const {
@@ -58,6 +60,7 @@ struct Aos32Rays {
 
 struct SoaRays {
   static constexpr int kPayloadWords = 0;
+  static constexpr bool kSharedOrigin = false;  // rays start anywhere (wavefront.cuh, CameraRaysT)
   const float4 *org_tmin;
   const float4 *dir_tmax;
   __device__ __forceinline__ void load(size_t i, float &ox, float &oy, float &oz, float &dx, float &dy,
@@ -140,7 +143,9 @@ int device_sm_count(int device) {
 //                 MINB REFILL PAIR128 LEAF_AGAIN DEFER NODE_UNROLL
 typedef Policy3<10, 24, true, 8, false, 2> DefaultPolicy;
 // The camera launch runs 9 CTAs per SM (56 registers: its AO-spawn retire step spills at 48) and, like the incoherent
-// launches, three node steps per exit check.
+// launches, three node steps per exit check.  Re-swept on H100 (80GB HBM3, 700 W) over the camera-relative layout and
+// the precomputed face normals: MINB 9/10 x NODE_UNROLL 2/3 all lie within 1 % of each other on the bench headline
+// (10 spills 32 B at 48 registers), so this row stays (DESIGN.md section 10).
 typedef Policy3<9, 32, true, 12, true, 3> CameraPolicy;
 typedef Policy3<10, 20, false, 12, false, 3> IncoherentPolicy;
 typedef Policy3<9, 32, false, 12, true, 3> IncoherentCameraPolicy;
@@ -149,6 +154,10 @@ typedef Policy3<9, 32, false, 12, true, 3> IncoherentCameraPolicy;
 typedef Policy3<8, 24, false, 8, true, 2> PathRadiancePolicy;
 // PairNode arrays above this size are not used (50 MB L2; the triangles want their share)
 constexpr size_t kPair128MaxBytes = (size_t)38 << 20;
+// The camera launch reads camera-relative copies of the PairNode and TriCM arrays (traverse3.cuh, from_origin) only
+// while the originals plus the copies fit in this: the AO launch that follows reads the originals, and the copies must
+// not evict them (the H100's L2 is two partitions of 25 MB)
+constexpr size_t kCameraRelMaxBytes = (size_t)24 << 20;
 
 static unsigned long long *next_cursor(const Accel *a, cudaStream_t s, cudaError_t *e) {
   // ring of 32 cursors: launches in flight on different streams never share one.  More than 32 traversal launches
@@ -170,9 +179,12 @@ static cudaError_t launch_fast3(const Accel *a, Rays rays, size_t n, Epi epi, co
   const size_t need_blocks = ((n + 31) / 32 + warps_per_block - 1) / warps_per_block;
   if (grid > need_blocks) grid = need_blocks;
   if (grid == 0) grid = 1;
-  const void *nodes = P::kPair128 ? static_cast<const void *>(a->d_pair) : static_cast<const void *>(a->d_wide);
+  const void *nodes = Rays::kSharedOrigin ? static_cast<const void *>(a->d_pair_rel)
+                     : P::kPair128        ? static_cast<const void *>(a->d_pair)
+                                          : static_cast<const void *>(a->d_wide);
+  const TriCM *tris = Rays::kSharedOrigin ? a->d_tris_rel : a->d_tris_cm;
   traverse_fast3_kernel<Rays, DEPTH, COUNT, P, Epi><<<(unsigned)grid, kTraverseBlock, 0, s>>>(
-      nodes, a->d_tris_cm, rays, n, epi, opt, flags, cursor, d_counts, n_ptr);
+      nodes, tris, rays, n, epi, opt, flags, cursor, d_counts, n_ptr);
   return cudaGetLastError();
 }
 
@@ -290,15 +302,22 @@ static int launch_fused(const Accel *a, Rays rays, size_t n, const unsigned long
   return launch_fast3_any<Rays, false, P>(a, rays, n, epi, opt, flags, nullptr, n_ptr, s);
 }
 
-// Camera rays, generated inside the kernel (no generator kernel, no primary queue)
-int launch_traverse_camera_fused(const Accel *a, const Wave &w, const nrt_ao_params &p, unsigned long long slot0,
-                                 size_t count, float *d_accum, unsigned long long *d_wave_counters,
+// Camera rays, generated inside the kernel (no generator kernel, no primary queue).  On the PairNode path they read
+// camera-relative copies of the nodes and triangles while the originals and the copies together stay well inside one
+// half of the L2 (kCameraRelMaxBytes); the caller orders `s` after every earlier pass that may still read the copies.
+int launch_traverse_camera_fused(Accel *a, const Wave &w, const nrt_ao_params &p, unsigned long long slot0, size_t count,
+                                 const float4 *d_face_n, float *d_accum, unsigned long long *d_wave_counters,
                                  const TraceOptions16 &opt, uint32_t flags, cudaStream_t s) {
-  PrimaryToAoEpilogue epi{p, w, a->d_verts, a->d_faces, d_accum, d_wave_counters};
+  PrimaryToAoEpilogue epi{p, w, d_face_n, d_accum, d_wave_counters};
   if (count == 0) return NRT_OK;
   if (a->n_wide * sizeof(PairNode) > kPair128MaxBytes)
-    return launch_fast3_any<CameraRays, false, IncoherentCameraPolicy>(a, CameraRays(p, slot0), count, epi, opt, flags, nullptr,
-                                                                       nullptr, s);
+    return launch_fast3_any<CameraRaysAbs, false, IncoherentCameraPolicy>(a, CameraRaysAbs(p, slot0), count, epi, opt, flags,
+                                                                          nullptr, nullptr, s);
+  if (2 * (a->n_wide * sizeof(PairNode) + (size_t)a->n_prims * sizeof(TriCM)) > kCameraRelMaxBytes)
+    return launch_fast3_any<CameraRaysAbs, false, CameraPolicy>(a, CameraRaysAbs(p, slot0), count, epi, opt, flags, nullptr,
+                                                                nullptr, s);
+  const int rc = camera_relative_layout(a, p.cam, s);
+  if (rc != NRT_OK) return rc;
   return launch_fast3_any<CameraRays, false, CameraPolicy>(a, CameraRays(p, slot0), count, epi, opt, flags, nullptr, nullptr, s);
 }
 

@@ -138,13 +138,18 @@ __device__ __forceinline__ void camera_ray(const float *cam, uint32_t width, uin
 // divisions replaced by multiplications (slot0 is a multiple of the per-tile slot count: waves are whole tiles), and
 // what the retire step needs again -- direction, pixel, sample, accumulation index -- travels as the ray's payload
 // (6 words the kernel parks in thread-local memory) instead of being recomputed.
-struct CameraRays {
+// SHARED_ORIGIN: the loader's kSharedOrigin, which every ray loader has -- true: all rays start at p.cam[0..2] and the
+// launch passes the nodes and triangles relative to that origin (Accel::d_pair_rel / d_tris_rel), so the traversal
+// kernel does not subtract it again (traverse3.cuh, from_origin).
+template <bool SHARED_ORIGIN>
+struct CameraRaysT {
   static constexpr int kPayloadWords = 6;
+  static constexpr bool kSharedOrigin = SHARED_ORIGIN;
   nrt_ao_params p;
   uint32_t k0;  // slot0 / per_tile: ordinal (within the shard) of the wave's first tile
   FastDiv per_tile, tile_pix, bw, tiles_x;
   uint32_t packed;
-  __host__ CameraRays(const nrt_ao_params &pp, unsigned long long slot0) : p(pp) {
+  __host__ CameraRaysT(const nrt_ao_params &pp, unsigned long long slot0) : p(pp) {
     const uint32_t tp = pp.tile_w * pp.tile_h;
     per_tile = FastDiv(tp * pp.spp);
     tile_pix = FastDiv(tp);
@@ -200,22 +205,34 @@ struct CameraRays {
     }
   }
 };
+typedef CameraRaysT<true> CameraRays;      // over the camera-relative copies
+typedef CameraRaysT<false> CameraRaysAbs;  // over the accel's own arrays
 
-// One cosine-hemisphere AO ray from a primary hit.
-__device__ __forceinline__ void make_ao_ray(const nrt_ao_params &p, uint32_t pix, uint32_t smp, float4 o, float4 d,
-                                            float t, uint32_t prim, const float *__restrict__ verts,
-                                            const uint32_t *__restrict__ faces, float4 &o4, float4 &d4) {
-  const float Px = o.x + d.x * t, Py = o.y + d.y * t, Pz = o.z + d.z * t;
+// Unit normalize(cross(v1 - v0, v2 - v0)) of a triangle (zero for a degenerate one) and twice its area.
+__device__ __forceinline__ void geometric_normal(const float *__restrict__ verts, const uint32_t *__restrict__ faces,
+                                                 uint32_t prim, float &nx, float &ny, float &nz, float &area2) {
   const uint32_t f0 = faces[3 * (size_t)prim], f1 = faces[3 * (size_t)prim + 1], f2 = faces[3 * (size_t)prim + 2];
   const float *p0 = verts + 3 * (size_t)f0, *p1 = verts + 3 * (size_t)f1, *p2 = verts + 3 * (size_t)f2;
   const float e1x = p1[0] - p0[0], e1y = p1[1] - p0[1], e1z = p1[2] - p0[2];
   const float e2x = p2[0] - p0[0], e2y = p2[1] - p0[1], e2z = p2[2] - p0[2];
-  float nx = e1y * e2z - e1z * e2y, ny = e1z * e2x - e1x * e2z, nz = e1x * e2y - e1y * e2x;
-  float ln = sqrtf(nx * nx + ny * ny + nz * nz);
-  ln = ln > 0.0f ? 1.0f / ln : 0.0f;
-  nx *= ln;
-  ny *= ln;
-  nz *= ln;
+  nx = e1y * e2z - e1z * e2y;
+  ny = e1z * e2x - e1x * e2z;
+  nz = e1x * e2y - e1y * e2x;
+  area2 = sqrtf(nx * nx + ny * ny + nz * nz);
+  const float il = area2 > 0.0f ? 1.0f / area2 : 0.0f;
+  nx *= il;
+  ny *= il;
+  nz *= il;
+}
+
+// One cosine-hemisphere AO ray from a primary hit.  normals[prim]: geometric_normal() of the primitive, computed once
+// per accel (Accel::d_face_n), so that the spawn needs one 128-bit load instead of two dependent rounds of gathers.
+__device__ __forceinline__ void make_ao_ray(const nrt_ao_params &p, uint32_t pix, uint32_t smp, float4 o, float4 d,
+                                            float t, uint32_t prim, const float4 *__restrict__ normals, float4 &o4,
+                                            float4 &d4) {
+  const float Px = o.x + d.x * t, Py = o.y + d.y * t, Pz = o.z + d.z * t;
+  const float4 n = __ldg(normals + prim);
+  float nx = n.x, ny = n.y, nz = n.z;
   if (nx * d.x + ny * d.y + nz * d.z > 0.0f) {
     nx = -nx;
     ny = -ny;
@@ -260,8 +277,7 @@ struct PrimaryToAoEpilogue {
   static constexpr bool kAnyHit = false;
   nrt_ao_params p;
   Wave w;
-  const float *verts;
-  const uint32_t *faces;
+  const float4 *normals;
   float *accum;
   unsigned long long *counters;  // [0] AO rays of this wave
   __device__ __forceinline__ void operator()(bool retiring, size_t ray_idx, float t, float u, float v, uint32_t prim,
@@ -280,7 +296,7 @@ struct PrimaryToAoEpilogue {
         const float4 rd = make_float4(__uint_as_float(payload[0]), __uint_as_float(payload[1]),
                                       __uint_as_float(payload[2]), p.ray_max_t);
         if (t < max_t) {
-          make_ao_ray(p, pix, smp, ro, rd, t, prim, verts, faces, o4, d4);
+          make_ao_ray(p, pix, smp, ro, rd, t, prim, normals, o4, d4);
           make = true;
         } else {
           atomicAdd(accum + acc, 1.0f);
@@ -332,22 +348,6 @@ struct PathQueues {
   float4 *sh_contrib_pix;
   float4 *weight;  // per path: throughput rgb
 };
-
-__device__ __forceinline__ void geometric_normal(const float *__restrict__ verts, const uint32_t *__restrict__ faces,
-                                                 uint32_t prim, float &nx, float &ny, float &nz, float &area2) {
-  const uint32_t f0 = faces[3 * (size_t)prim], f1 = faces[3 * (size_t)prim + 1], f2 = faces[3 * (size_t)prim + 2];
-  const float *p0 = verts + 3 * (size_t)f0, *p1 = verts + 3 * (size_t)f1, *p2 = verts + 3 * (size_t)f2;
-  const float e1x = p1[0] - p0[0], e1y = p1[1] - p0[1], e1z = p1[2] - p0[2];
-  const float e2x = p2[0] - p0[0], e2y = p2[1] - p0[1], e2z = p2[2] - p0[2];
-  nx = e1y * e2z - e1z * e2y;
-  ny = e1z * e2x - e1x * e2z;
-  nz = e1x * e2y - e1y * e2x;
-  area2 = sqrtf(nx * nx + ny * ny + nz * nz);
-  const float il = area2 > 0.0f ? 1.0f / area2 : 0.0f;
-  nx *= il;
-  ny *= il;
-  nz *= il;
-}
 
 // 16 floats per material, the tinyobj fields the reference reads (main.cc:884-892)
 struct PathMaterial {
