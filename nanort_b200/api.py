@@ -268,7 +268,8 @@ class Comm:
             pass
 
     def RenderAO(self, accel, params: AoParams, d_frame_full_ptr, stream=None, want_result=True):
-        """nrt_render_ao_sharded: this rank's tiles + framebuffer all-gather; every rank's d_frame_full holds the frame."""
+        """nrt_render_ao_sharded: this rank's tiles + framebuffer all-gather; every rank's d_frame_full holds the frame.
+        Calls on one communicator may be enqueued on any streams: they run one after the other on the device."""
         res = AoResult()
         _check(lib().nrt_render_ao_sharded(accel._h, self._h, C.byref(params), C.c_void_p(d_frame_full_ptr),
                                            C.byref(res) if want_result else None, C.c_void_p(stream) if stream else None))
@@ -410,7 +411,8 @@ class BVHAccel:
 
     def TraverseDevice(self, d_rays_ptr, n, d_hits_ptr, d_mask_ptr=None, options=None, flags=TRAVERSE_FAST,
                        stream=None):
-        """Device-pointer form (nrt_traverse_device); pointers are ints (e.g. torch.Tensor.data_ptr())."""
+        """Device-pointer form (nrt_traverse_device); pointers are ints (e.g. torch.Tensor.data_ptr()).  Asynchronous on
+        `stream`: any number of calls of one accel may be in flight on any streams, next to its AO and path passes."""
         _check(lib().nrt_traverse_device(self._h, C.c_void_p(d_rays_ptr), int(n), C.c_void_p(d_hits_ptr),
                                          C.c_void_p(d_mask_ptr) if d_mask_ptr else None, _p(options), int(flags),
                                          C.c_void_p(stream) if stream else None))
@@ -442,7 +444,8 @@ class BVHAccel:
         return n_p.value, n_a.value
 
     def RenderPath(self, params: PathParams, d_accum_rgb_ptr, stream=None, want_result=True):
-        """Wavefront path tracing pass (nrt_render_path_device)."""
+        """Wavefront path tracing pass (nrt_render_path_device).  Passes on one accel (AO, path passes, PathBounce) may
+        be enqueued on any streams: they run one after the other on the device."""
         res = PathResult()
         _check(lib().nrt_render_path_device(self._h, C.byref(params), C.c_void_p(d_accum_rgb_ptr),
                                             C.byref(res) if want_result else None,
@@ -510,6 +513,7 @@ class BVHAccel:
         return int(nc.value), int(ns.value)
 
     def RenderAO(self, params: AoParams, d_accum_ptr, stream=None, want_result=True):
+        """Primary + AO pass (nrt_render_ao_device); ordered on the device with the accel's other passes like RenderPath."""
         res = AoResult()
         _check(lib().nrt_render_ao_device(self._h, C.byref(params), C.c_void_p(d_accum_ptr),
                                           C.byref(res) if want_result else None,
@@ -710,7 +714,8 @@ class BVHAccelF64:
         return hits, mask
 
     def TraverseDevice(self, d_rays_ptr, n, d_hits_ptr, d_mask_ptr=None, options=None, flags=0, stream=None):
-        """Device-pointer form (nrt_traverse_f64_device): 72-byte rays in, 32-byte records out."""
+        """Device-pointer form (nrt_traverse_f64_device): 72-byte rays in, 32-byte records out.  Asynchronous on
+        `stream`: any number of calls of one accel may be in flight on any streams."""
         _check(lib().nrt_traverse_f64_device(self._h, C.c_void_p(d_rays_ptr), int(n), C.c_void_p(d_hits_ptr),
                                              C.c_void_p(d_mask_ptr) if d_mask_ptr else None, _p(options), int(flags),
                                              C.c_void_p(stream) if stream else None))

@@ -52,7 +52,9 @@ static void destroy(Accel *a) {
   cudaFree(a->d_pair_rel);
   cudaFree(a->d_tris_rel);
   cudaFree(a->d_face_n);
-  if (a->ao_pass_done) cudaEventDestroy(a->ao_pass_done);
+  if (a->pass_done) cudaEventDestroy(a->pass_done);
+  for (cudaEvent_t e : a->ring_done)
+    if (e) cudaEventDestroy(e);
   cudaFree(a->d_prim_boxes);
   cudaFree(a->d_prim_data);
   cudaFree(a->d_wave);
@@ -435,6 +437,8 @@ int nrt_nodes(nrt_accel *h, const void **nodes_40B, size_t *n_nodes, const uint3
   return NRT_OK;
 }
 
+// Any number of calls of one accel may be in flight on any streams: fast launches take their ray cursor from the
+// accel's ring, whose slots are ordered on the device by Accel::ring_done (traverse.cu:launch_fast3_any).
 int nrt_traverse_device(const nrt_accel *h, const void *d_rays_36B, size_t n_rays, void *d_hits_16B,
                         uint8_t *d_hit_mask, const void *trace_opts_16B, uint32_t flags, void *stream) {
   if (!h || (n_rays && (!d_rays_36B || !d_hits_16B))) {

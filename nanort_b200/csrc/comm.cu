@@ -75,6 +75,9 @@ struct Comm {
   int rank = 0, world = 1, device = 0;
   float *d_gather = nullptr;  // world x slot_floats, tile-major; slot `rank` is this rank's accumulation target
   size_t gather_floats = 0;
+  // recorded after the last kernel of every sharded pass that reads d_gather; the next pass on this communicator
+  // waits on it (any stream) before it zeroes its slot.  d_gather, gather_floats and the event are guarded by mu.
+  cudaEvent_t gather_done = nullptr;
   std::mutex mu;
 };
 
@@ -157,6 +160,7 @@ void nrt_comm_free(nrt_comm *h) {
   cudaDeviceSynchronize();
   if (c->comm && nccl().CommDestroy) nccl().CommDestroy(c->comm);
   cudaFree(c->d_gather);
+  if (c->gather_done) cudaEventDestroy(c->gather_done);
   delete c;
 }
 
@@ -192,13 +196,16 @@ int nrt_render_ao_sharded(const nrt_accel *accel, nrt_comm *h, const nrt_ao_para
   p.n_shards = (uint32_t)c->world;
   p.flags = (p.flags & ~NRT_AO_UNFUSED) | NRT_AO_PACKED_TILES;
   NRT_DEVICE(c->device);
+  // c->mu orders the enqueueing; gather_done makes this pass wait on the device for the previous pass on this
+  // communicator, which may still accumulate into or unpack d_gather on another stream
   std::lock_guard<std::mutex> lock(c->mu);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (!c->gather_done) NRT_CUDA(cudaEventCreateWithFlags(&c->gather_done, cudaEventDisableTiming));
   const uint32_t tiles_x = (p.width + p.tile_w - 1) / p.tile_w, tiles_y = (p.height + p.tile_h - 1) / p.tile_h;
   const size_t n_tiles = (size_t)tiles_x * tiles_y;
   const size_t slot_floats = ((n_tiles + c->world - 1) / c->world) * (size_t)p.tile_w * p.tile_h;  // equal for all ranks
   if (c->gather_floats < slot_floats * c->world) {
-    NRT_CUDA(cudaStreamSynchronize(s));
+    NRT_CUDA(cudaEventSynchronize(c->gather_done));
     cudaFree(c->d_gather);
     c->d_gather = nullptr;
     c->gather_floats = 0;
@@ -206,6 +213,8 @@ int nrt_render_ao_sharded(const nrt_accel *accel, nrt_comm *h, const nrt_ao_para
     c->gather_floats = slot_floats * c->world;
   }
   float *mine = c->d_gather + (size_t)c->rank * slot_floats;
+  NRT_CUDA(cudaStreamWaitEvent(s, c->gather_done, 0));
+  const RecordOnExit gather_done{c->gather_done, s};
   NRT_CUDA(cudaMemsetAsync(mine, 0, sizeof(float) * slot_floats, s));
   int rc = run_ao_pass_internal(accel, &p, mine, res, stream);
   if (rc != NRT_OK) return rc;

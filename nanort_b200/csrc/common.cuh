@@ -170,9 +170,10 @@ struct Accel {
   uint32_t rel_origin[3] = {0, 0, 0};
   // unit geometric normal per primitive (float4, w unused), read by the AO spawn; derived on the first AO pass
   float4 *d_face_n = nullptr;
-  // recorded after the last launch of every AO pass; the next pass waits on it (any stream), so that the pass scratch
-  // (d_wave, d_counters[2..6]) and the camera-relative copies are never rewritten while a pass still reads them
-  cudaEvent_t ao_pass_done = nullptr;
+  // recorded after the last launch of every AO pass, path pass and path bounce; the next one waits on it (any stream),
+  // so that the pass scratch (d_wave, d_counters[2..6] and [48..54]) and the camera-relative copies are never
+  // rewritten while a pass still reads them
+  cudaEvent_t pass_done = nullptr;
   // host mirrors (lazy)
   std::vector<Node40> h_nodes;
   std::vector<uint32_t> h_indices;
@@ -209,11 +210,17 @@ struct Accel {
   // wavefront pass scratch (render.cu)
   void *d_wave = nullptr;
   size_t wave_bytes = 0;
-  // device counter block (96 words): [0..7] misc, [8..9] visit counts, [16..47] ring of ray cursors (one per
-  // in-flight traversal launch, so launches on different streams never share a cursor), [48..54] path tracer,
-  // [64..79] count / lane-stat scratch, [80..95] the small slots' ray cursors
+  // device counter block (96 words): [0..7] misc, [8..9] visit counts, [16..47] ring of ray cursors, [48..54] path
+  // tracer, [64..79] count / lane-stat scratch, [80..95] the small slots' ray cursors
   uint64_t *d_counters = nullptr;
-  mutable std::atomic<uint32_t> cursor_ring{0};
+  // the ring: persistent traversal launches take the next of kRingSlots cursors d_counters[16 + k].  ring_done[k] is
+  // recorded after the last launch that used cursor k, and the next launch on cursor k makes its stream wait for it,
+  // so any number of launches in flight on any streams never share a cursor.  cursor_ring and the events are guarded
+  // by ring_mu (taken after host_mu, never before it).
+  static constexpr uint32_t kRingSlots = 32;
+  mutable std::mutex ring_mu;
+  mutable uint32_t cursor_ring = 0;
+  mutable cudaEvent_t ring_done[kRingSlots] = {};
 };
 
 void set_error(const std::string &msg);
@@ -254,6 +261,31 @@ struct DeviceGuard {
 #define NRT_DEVICE(dev)            \
   nrt::DeviceGuard _nrt_dg((dev)); \
   NRT_CUDA(_nrt_dg.err)
+
+// Passes on one accel (AO passes, path passes, path bounces) share its pass scratch.  Under host_mu, a pass calls
+// wait_previous_pass before it enqueues anything and holds a RecordOnExit for as long as it enqueues, so that every
+// pass runs on the device after the one enqueued before it, whatever streams the two are on.
+inline int wait_previous_pass(Accel *a, cudaStream_t s) {
+  if (!a->pass_done) NRT_CUDA(cudaEventCreateWithFlags(&a->pass_done, cudaEventDisableTiming));
+  NRT_CUDA(cudaStreamWaitEvent(s, a->pass_done, 0));
+  return NRT_OK;
+}
+struct RecordOnExit {
+  cudaEvent_t e;
+  cudaStream_t s;
+  ~RecordOnExit() { cudaEventRecord(e, s); }
+};
+// the pass scratch grows only after the pass that last used it has finished
+inline int grow_wave(Accel *a, size_t need) {
+  if (a->wave_bytes >= need) return NRT_OK;
+  NRT_CUDA(cudaEventSynchronize(a->pass_done));
+  cudaFree(a->d_wave);
+  a->d_wave = nullptr;
+  a->wave_bytes = 0;
+  NRT_CUDA(cudaMalloc(&a->d_wave, need));
+  a->wave_bytes = need;
+  return NRT_OK;
+}
 
 __host__ __device__ inline TraceOptions16 default_trace_options() {
   TraceOptions16 o;

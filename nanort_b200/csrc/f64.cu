@@ -66,8 +66,13 @@ struct AccelF64 {
   size_t stage = 0;
   // fast-path layout (f64_fast.cuh), derived on the first fast Traverse
   void *d_pair = nullptr, *d_tris_fast = nullptr;
-  unsigned long long *d_cursor = nullptr;  // ring of 8 ray-pool cursors
+  // ring of 8 ray-pool cursors: cursor_done[k] is recorded after the last launch that used cursor k, and the next
+  // launch on cursor k makes its stream wait for it, so any number of launches in flight never share a cursor.
+  // cursor_next and the events are guarded by mu.
+  static constexpr unsigned kCursors = 8;
+  unsigned long long *d_cursor = nullptr;
   unsigned cursor_next = 0;
+  cudaEvent_t cursor_done[kCursors] = {};
   bool fast_ready = false;
   std::mutex mu;
   // small reference-order calls (the facade's one-ray Traverse): zero-copy slots as in Accel::SmallSlot
@@ -103,6 +108,8 @@ void destroy_f64(AccelF64 *a) {
   cudaFree(a->d_pair);
   cudaFree(a->d_tris_fast);
   cudaFree(a->d_cursor);
+  for (cudaEvent_t e : a->cursor_done)
+    if (e) cudaEventDestroy(e);
   if (a->stream) cudaStreamDestroy(a->stream);
   delete a;
 }
@@ -246,7 +253,8 @@ int derive_fast_layout_f64(AccelF64 *a) {
   const size_t n_pair = n_branch > 0 ? n_branch : 1;
   if (e == cudaSuccess && rc == NRT_OK) e = cudaMalloc(&a->d_pair, sizeof(PairNodeD) * n_pair);
   if (e == cudaSuccess && rc == NRT_OK) e = cudaMalloc(&a->d_tris_fast, sizeof(TriD) * (size_t)a->n_prims);
-  if (e == cudaSuccess && rc == NRT_OK && !a->d_cursor) e = cudaMalloc(&a->d_cursor, sizeof(unsigned long long) * 8);
+  if (e == cudaSuccess && rc == NRT_OK && !a->d_cursor)
+    e = cudaMalloc(&a->d_cursor, sizeof(unsigned long long) * AccelF64::kCursors);
   if (e == cudaSuccess && rc == NRT_OK) {
     f64_tris_kernel<<<(a->n_prims + 255) / 256, 256, 0, s>>>(a->d_indices, a->d_faces, a->d_verts, a->n_prims,
                                                             static_cast<TriD *>(a->d_tris_fast));
@@ -267,11 +275,17 @@ int derive_fast_layout_f64(AccelF64 *a) {
   return NRT_OK;
 }
 
+// Called under a->mu, which orders taking the cursor, waiting for its previous launch, zeroing it, launching and
+// recording the same way on the host and on the device.
 template <int DEPTH>
 cudaError_t launch_fast_f64(AccelF64 *a, const Ray72 *d_rays, size_t m, Hit32 *d_hits, uint8_t *d_mask,
                             const TraceOptions16 &opt, uint32_t flags, cudaStream_t s) {
-  unsigned long long *cursor = a->d_cursor + (a->cursor_next++ & 7u);
-  cudaError_t e = cudaMemsetAsync(cursor, 0, sizeof(unsigned long long), s);
+  const unsigned k = a->cursor_next++ % AccelF64::kCursors;
+  unsigned long long *cursor = a->d_cursor + k;
+  cudaEvent_t &done = a->cursor_done[k];
+  cudaError_t e = done ? cudaSuccess : cudaEventCreateWithFlags(&done, cudaEventDisableTiming);
+  if (e == cudaSuccess) e = cudaStreamWaitEvent(s, done, 0);
+  if (e == cudaSuccess) e = cudaMemsetAsync(cursor, 0, sizeof(unsigned long long), s);
   if (e != cudaSuccess) return e;
   size_t grid = (size_t)device_sm_count(a->device) * kFastBlocksPerSmD;  // persistent: every SM holds its complement
   const size_t need = ((m + 31) / 32 + kFastBlockD / 32 - 1) / (kFastBlockD / 32);
@@ -280,7 +294,9 @@ cudaError_t launch_fast_f64(AccelF64 *a, const Ray72 *d_rays, size_t m, Hit32 *d
   traverse_fast_f64_kernel<DEPTH><<<(unsigned)grid, kFastBlockD, 0, s>>>(
       static_cast<const PairNodeD *>(a->d_pair), static_cast<const TriD *>(a->d_tris_fast), d_rays, m, d_hits, d_mask, opt,
       flags, cursor);
-  return cudaGetLastError();
+  e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  return cudaEventRecord(done, s);
 }
 
 }  // namespace
@@ -665,6 +681,8 @@ int nrt_traverse_f64(const nrt_accel_f64 *h, const void *rays_72B, size_t n_rays
   return NRT_OK;
 }
 
+// Any number of calls of one accel may be in flight on any streams (launch_fast_f64 orders the cursor ring's slots
+// on the device).
 int nrt_traverse_f64_device(const nrt_accel_f64 *h, const void *d_rays_72B, size_t n_rays, void *d_hits_32B,
                             uint8_t *d_hit_mask, const void *trace_opts_16B, uint32_t flags, void *stream) {
   if (!h || (n_rays && (!d_rays_72B || !d_hits_32B))) {
@@ -675,7 +693,7 @@ int nrt_traverse_f64_device(const nrt_accel_f64 *h, const void *d_rays_72B, size
   AccelF64 *a = const_cast<AccelF64 *>(reinterpret_cast<const AccelF64 *>(h));
   TraceOptions16 opt = default_trace_options();
   if (trace_opts_16B) memcpy(&opt, trace_opts_16B, sizeof(opt));
-  std::lock_guard<std::mutex> lock(a->mu);  // lazy layout + the cursor ring
+  std::lock_guard<std::mutex> lock(a->mu);  // lazy layout + the cursor ring (launch_fast_f64)
   NRT_DEVICE(a->device);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const Ray72 *d_r = static_cast<const Ray72 *>(d_rays_72B);

@@ -91,8 +91,12 @@ extern "C" int nrt_render_path_device(const nrt_accel *h, const nrt_path_params 
     return NRT_ERR_INVALID;
   }
   NRT_DEVICE(a->device);
-  std::lock_guard<std::mutex> lock(a->host_mu);  // d_wave / d_counters are per-accel scratch (see render.cu)
+  // d_wave / d_counters[48..54] are per-accel scratch, shared with AO passes and path bounces: the pass waits on the
+  // device for the previous pass on this accel (render.cu)
+  std::lock_guard<std::mutex> lock(a->host_mu);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (const int rc = wait_previous_pass(a, s)) return rc;
+  const RecordOnExit pass_done{a->pass_done, s};
   const uint32_t tiles_x = (p.width + p.tile_w - 1) / p.tile_w, tiles_y = (p.height + p.tile_h - 1) / p.tile_h;
   const uint32_t n_tiles = tiles_x * tiles_y;
   const uint32_t my_tiles = n_tiles > p.shard ? (n_tiles - p.shard + p.n_shards - 1) / p.n_shards : 0;
@@ -105,13 +109,7 @@ extern "C" int nrt_render_path_device(const nrt_accel *h, const nrt_path_params 
   // per path: 2 radiance queues (32 + 4 B each), shadow queue (48 B), weight (16 B)
   const size_t per_path = 2 * (2 * sizeof(float4) + 4) + 3 * sizeof(float4) + sizeof(float4);
   const size_t need = (size_t)cap * per_path + 256;
-  if (a->wave_bytes < need) {
-    cudaFree(a->d_wave);
-    a->d_wave = nullptr;
-    a->wave_bytes = 0;
-    NRT_CUDA(cudaMalloc(&a->d_wave, need));
-    a->wave_bytes = need;
-  }
+  if (const int rc = grow_wave(a, need)) return rc;
   PathQueues q;
   {
     char *b = static_cast<char *>(a->d_wave);
@@ -233,8 +231,11 @@ extern "C" int nrt_path_bounce_device(const nrt_accel *h, const nrt_path_params 
   if (n_shadow) *n_shadow = 0;
   if (n_rays == 0) return NRT_OK;
   NRT_DEVICE(a->device);
+  // d_counters[48..51] are the pass scratch of nrt_render_path_device too: ordered like a pass
   std::lock_guard<std::mutex> lock(a->host_mu);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (const int rc = wait_previous_pass(a, s)) return rc;
+  const RecordOnExit pass_done{a->pass_done, s};
   PathQueues q;
   q.org_tmin[0] = static_cast<float4 *>(const_cast<void *>(d_org_tmin));
   q.dir_tmax[0] = static_cast<float4 *>(const_cast<void *>(d_dir_tmax));

@@ -193,19 +193,14 @@ static int run_ao_pass(const nrt_accel *h, const nrt_ao_params *pp, float *d_acc
     return NRT_ERR_INVALID;
   }
   NRT_DEVICE(a->device);
-  // d_wave and d_counters[2..6] are per-accel scratch: concurrent passes on ONE accel are serialised (passes on
-  // different accels, e.g. one per GPU, run concurrently)
+  // d_wave and d_counters[2..6] are per-accel scratch: passes on ONE accel run one after the other on the device
+  // (passes on different accels, e.g. one per GPU, run concurrently).  host_mu orders the enqueueing; pass_done makes
+  // this pass wait for the previous AO or path pass on this accel, which may still run on another stream, so that
+  // nothing it reads (the wave scratch, the counters, the camera-relative copies) is rewritten before it has finished
   std::lock_guard<std::mutex> lock(a->host_mu);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  // host_mu orders the enqueueing only: the previous pass on this accel may still run on another stream, and nothing
-  // it reads (the wave scratch, the counters, the camera-relative copies) is rewritten before it has finished
-  if (!a->ao_pass_done) NRT_CUDA(cudaEventCreateWithFlags(&a->ao_pass_done, cudaEventDisableTiming));
-  NRT_CUDA(cudaStreamWaitEvent(s, a->ao_pass_done, 0));
-  struct RecordOnExit {
-    cudaEvent_t e;
-    cudaStream_t s;
-    ~RecordOnExit() { cudaEventRecord(e, s); }
-  } pass_done{a->ao_pass_done, s};
+  if (const int rc = wait_previous_pass(a, s)) return rc;
+  const RecordOnExit pass_done{a->pass_done, s};
   if (!a->d_face_n) {
     NRT_CUDA(cudaMalloc(&a->d_face_n, sizeof(float4) * (size_t)a->n_prims));
     face_normals_kernel<<<(a->n_prims + 255) / 256, 256, 0, s>>>(a->d_verts, a->d_faces, a->n_prims, a->d_face_n);
@@ -225,13 +220,7 @@ static int run_ao_pass(const nrt_accel *h, const nrt_ao_params *pp, float *d_acc
   const unsigned long long cap = std::min<unsigned long long>(total_slots, tiles_per_wave * per_tile);
   const size_t per_ray = 2 * sizeof(float4) + sizeof(Hit16) + 4 + 2 * sizeof(float4) + 4 + sizeof(Hit16);
   const size_t need = (size_t)cap * per_ray + 256;
-  if (a->wave_bytes < need) {
-    cudaFree(a->d_wave);
-    a->d_wave = nullptr;
-    a->wave_bytes = 0;
-    NRT_CUDA(cudaMalloc(&a->d_wave, need));
-    a->wave_bytes = need;
-  }
+  if (const int rc = grow_wave(a, need)) return rc;
   Wave w;
   {
     char *b = static_cast<char *>(a->d_wave);

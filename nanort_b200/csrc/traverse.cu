@@ -159,16 +159,6 @@ constexpr size_t kPair128MaxBytes = (size_t)38 << 20;
 // not evict them (the H100's L2 is two partitions of 25 MB)
 constexpr size_t kCameraRelMaxBytes = (size_t)24 << 20;
 
-static unsigned long long *next_cursor(const Accel *a, cudaStream_t s, cudaError_t *e) {
-  // ring of 32 cursors: launches in flight on different streams never share one.  More than 32 traversal launches
-  // of ONE accel in flight at once would alias; every entry point that draws from the ring keeps at most 3 (the
-  // small-call path, which many host threads use at once, has one cursor per slot instead: Accel::kSmallCursor0).
-  unsigned long long *cursor =
-      reinterpret_cast<unsigned long long *>(a->d_counters) + 16 + (a->cursor_ring.fetch_add(1) & 31u);
-  *e = cudaMemsetAsync(cursor, 0, sizeof(unsigned long long), s);
-  return cursor;
-}
-
 template <class Rays, int DEPTH, bool COUNT, class P, class Epi>
 static cudaError_t launch_fast3(const Accel *a, Rays rays, size_t n, Epi epi, const TraceOptions16 &opt,
                                 uint32_t flags, unsigned long long *cursor, unsigned long long *d_counts,
@@ -194,6 +184,22 @@ static cudaError_t launch_fast3(const Accel *a, Rays rays, size_t n, Epi epi, co
 static bool needs_deep_stack(const Accel *a) { return a->stats.max_tree_depth + 2 > 64u; }
 
 template <class Rays, bool COUNT, class P, class Epi>
+static int launch_fast3_cursor(const Accel *a, Rays rays, size_t n, Epi epi, const TraceOptions16 &opt, uint32_t flags,
+                               unsigned long long *d_counts, const unsigned long long *n_ptr, cudaStream_t s,
+                               unsigned long long *cursor) {
+  NRT_CUDA(cudaMemsetAsync(cursor, 0, sizeof(unsigned long long), s));
+  cudaError_t e;
+  if (needs_deep_stack(a))
+    e = launch_fast3<Rays, 512, COUNT, P>(a, rays, n, epi, opt, flags, cursor, d_counts, n_ptr, s);
+  else
+    e = launch_fast3<Rays, 64, COUNT, P>(a, rays, n, epi, opt, flags, cursor, d_counts, n_ptr, s);
+  NRT_CUDA(e);
+  return NRT_OK;
+}
+
+// `cursor`: a cursor the caller owns (the small-call slots: held until their launch has finished), or nullptr for the
+// next one of the accel's ring (Accel::ring_done)
+template <class Rays, bool COUNT, class P, class Epi>
 static int launch_fast3_any(const Accel *a, Rays rays, size_t n, Epi epi, const TraceOptions16 &opt, uint32_t flags,
                             unsigned long long *d_counts, const unsigned long long *n_ptr, cudaStream_t s,
                             unsigned long long *cursor = nullptr) {
@@ -201,17 +207,18 @@ static int launch_fast3_any(const Accel *a, Rays rays, size_t n, Epi epi, const 
     set_error("traverse: this accel has no triangle traversal layout");
     return NRT_ERR_INVALID;
   }
-  cudaError_t e;
-  if (cursor)
-    e = cudaMemsetAsync(cursor, 0, sizeof(unsigned long long), s);
-  else
-    cursor = next_cursor(a, s, &e);
-  NRT_CUDA(e);
-  if (needs_deep_stack(a))
-    e = launch_fast3<Rays, 512, COUNT, P>(a, rays, n, epi, opt, flags, cursor, d_counts, n_ptr, s);
-  else
-    e = launch_fast3<Rays, 64, COUNT, P>(a, rays, n, epi, opt, flags, cursor, d_counts, n_ptr, s);
-  NRT_CUDA(e);
+  if (cursor) return launch_fast3_cursor<Rays, COUNT, P>(a, rays, n, epi, opt, flags, d_counts, n_ptr, s, cursor);
+  // taking the slot, waiting for its previous launch, zeroing the cursor, launching and recording happen under one
+  // lock, so they are in the same order on the host and on the device
+  std::lock_guard<std::mutex> lock(a->ring_mu);
+  const uint32_t k = a->cursor_ring++ % Accel::kRingSlots;
+  cudaEvent_t &done = a->ring_done[k];
+  if (!done) NRT_CUDA(cudaEventCreateWithFlags(&done, cudaEventDisableTiming));
+  NRT_CUDA(cudaStreamWaitEvent(s, done, 0));
+  cursor = reinterpret_cast<unsigned long long *>(a->d_counters) + 16 + k;
+  const int rc = launch_fast3_cursor<Rays, COUNT, P>(a, rays, n, epi, opt, flags, d_counts, n_ptr, s, cursor);
+  if (rc != NRT_OK) return rc;
+  NRT_CUDA(cudaEventRecord(done, s));
   return NRT_OK;
 }
 
