@@ -53,38 +53,21 @@ static void destroy(Accel *a) {
   cudaFree(a->d_tris_rel);
   cudaFree(a->d_face_n);
   if (a->pass_done) cudaEventDestroy(a->pass_done);
-  for (cudaEvent_t e : a->ring_done)
-    if (e) cudaEventDestroy(e);
   cudaFree(a->d_prim_boxes);
   cudaFree(a->d_prim_data);
   cudaFree(a->d_wave);
   cudaFree(a->d_counters);
-  for (int i = 0; i < 3; i++) {
-    cudaFree(a->d_stage_rays[i]);
-    cudaFree(a->d_stage_hits[i]);
-    cudaFree(a->d_stage_mask[i]);
-    if (a->streams[i]) cudaStreamDestroy(a->streams[i]);
-  }
-  for (int i = 0; i < Accel::kSmallSlots; i++) {
-    if (a->small[i].h) cudaFreeHost(a->small[i].h);
-    if (a->small[i].s) cudaStreamDestroy(a->small[i].s);
-  }
   delete a;
 }
 
 // Uploads geometry as tightly packed float3 vertices + faces.
-// Stream-ordered on a->streams[0], the (non-blocking) stream every build / layout kernel of this accel runs on: a
+// Stream-ordered on a->staging.stream(0), the (non-blocking) stream every build / layout kernel of this accel runs on: a
 // synchronous cudaMemcpy from pageable memory on the NULL stream may return before its DMA has finished, and
 // non-blocking streams do not order after the NULL stream.
 static int upload_geometry(Accel *a, const float *verts, size_t stride, size_t n_verts, const uint32_t *faces,
                            uint32_t n_prims) {
-  cudaStream_t s = a->streams[0];
-  if (n_verts == 0) {
-    uint32_t m = 0;
-    const size_t cnt = (size_t)n_prims * 3;
-    for (size_t i = 0; i < cnt; i++) m = std::max(m, faces[i]);
-    n_verts = (size_t)m + 1;
-  }
+  cudaStream_t s = a->staging.stream(0);
+  if (n_verts == 0) n_verts = infer_n_verts(faces, n_prims);
   a->n_verts = n_verts;
   a->n_prims = n_prims;
   NRT_CUDA(cudaMalloc(&a->d_verts, sizeof(float) * 3 * n_verts));
@@ -185,74 +168,17 @@ bool validate_foreign_tree64(const void *nodes_64B, size_t n_nodes, const uint32
   return validate_foreign_tree_t(static_cast<const Node64 *>(nodes_64B), n_nodes, indices, n_indices, n_prims, stats, why);
 }
 
-static int common_init(Accel *a) {
+size_t infer_n_verts(const uint32_t *faces, uint32_t n_prims) {
+  uint32_t m = 0;
+  for (size_t i = 0; i < (size_t)n_prims * 3; i++) m = std::max(m, faces[i]);
+  return (size_t)m + 1;
+}
+
+int common_init(Accel *a) {
   a->device = g_device;
   NRT_CUDA(cudaMalloc(&a->d_counters, 96 * sizeof(uint64_t)));
   NRT_CUDA(cudaMemset(a->d_counters, 0, 96 * sizeof(uint64_t)));
-  for (int i = 0; i < 3; i++) NRT_CUDA(cudaStreamCreateWithFlags(&a->streams[i], cudaStreamNonBlocking));
-  return NRT_OK;
-}
-
-static int ensure_staging(Accel *a, size_t chunk) {
-  if (a->stage_rays >= chunk) return NRT_OK;
-  for (int i = 0; i < 3; i++) {
-    cudaFree(a->d_stage_rays[i]);
-    cudaFree(a->d_stage_hits[i]);
-    cudaFree(a->d_stage_mask[i]);
-    a->d_stage_rays[i] = a->d_stage_hits[i] = a->d_stage_mask[i] = nullptr;
-  }
-  a->stage_rays = 0;
-  for (int i = 0; i < 3; i++) {
-    NRT_CUDA(cudaMalloc(&a->d_stage_rays[i], chunk * sizeof(Ray36)));
-    NRT_CUDA(cudaMalloc(&a->d_stage_hits[i], chunk * sizeof(Hit16)));
-    NRT_CUDA(cudaMalloc(&a->d_stage_mask[i], chunk));
-  }
-  a->stage_rays = chunk;
-  return NRT_OK;
-}
-
-// nrt_traverse for a handful of rays (the facade's per-ray Traverse, small packets from worker threads): see
-// Accel::SmallSlot.  The traversal kernels dereference the pinned host pointers directly (unified addressing).
-static int traverse_small(Accel *a, const void *rays, size_t n, void *hits_16B, uint8_t *hit_mask, const TraceOptions16 &opt,
-                          uint32_t flags) {
-  const size_t ray_bytes = (flags & NRT_TRAVERSE_RAY32) ? 32 : sizeof(Ray36);
-  const size_t off_hits = Accel::kSmallRays * sizeof(Ray36), off_mask = off_hits + Accel::kSmallRays * sizeof(Hit16);
-  int idx = -1;
-  {
-    std::unique_lock<std::mutex> lk(a->small_mu);
-    for (;;) {
-      for (int i = 0; i < Accel::kSmallSlots && idx < 0; i++)
-        if (!a->small[i].busy) idx = i;
-      if (idx >= 0) break;
-      a->small_cv.wait(lk);
-    }
-    a->small[idx].busy = true;
-  }
-  Accel::SmallSlot &sl = a->small[idx];
-  int rc = NRT_OK;
-  cudaError_t e = cudaSuccess;
-  if (!sl.h) e = cudaHostAlloc(&sl.h, off_mask + Accel::kSmallRays, cudaHostAllocPortable | cudaHostAllocMapped);
-  if (e == cudaSuccess && !sl.s) e = cudaStreamCreateWithFlags(&sl.s, cudaStreamNonBlocking);
-  if (e == cudaSuccess) {
-    char *hb = static_cast<char *>(sl.h);
-    memcpy(hb, rays, n * ray_bytes);
-    rc = launch_traverse(a, reinterpret_cast<const Ray36 *>(hb), n, reinterpret_cast<Hit16 *>(hb + off_hits),
-                         hit_mask ? reinterpret_cast<uint8_t *>(hb + off_mask) : nullptr, opt, flags, sl.s,
-                         reinterpret_cast<unsigned long long *>(a->d_counters) + Accel::kSmallCursor0 + idx);
-    e = cudaStreamSynchronize(sl.s);  // also on a failed launch: nothing of this call may be left in flight
-    if (rc == NRT_OK && e == cudaSuccess) {
-      memcpy(hits_16B, hb + off_hits, n * sizeof(Hit16));
-      if (hit_mask) memcpy(hit_mask, hb + off_mask, n);
-    }
-  }
-  {
-    std::lock_guard<std::mutex> lk(a->small_mu);
-    sl.busy = false;
-  }
-  a->small_cv.notify_one();
-  if (rc != NRT_OK) return rc;
-  NRT_CUDA(e);
-  return NRT_OK;
+  return a->staging.create_streams();
 }
 
 }  // namespace nrt
@@ -323,10 +249,10 @@ int nrt_build_ex(const float *verts, size_t stride_bytes, size_t n_verts, const 
   if (rc == NRT_OK) rc = upload_geometry(a, verts, stride_bytes, n_verts, faces, n_prims);
   if (rc == NRT_OK) {
     rc = (flags & NRT_BUILD_REFERENCE_TREE)
-             ? build_reference_tree_on_device(a, !(flags & NRT_BUILD_REFERENCE_CPP03_ORDER), a->streams[0])
-             : build_on_device(a, a->streams[0]);
+             ? build_reference_tree_on_device(a, !(flags & NRT_BUILD_REFERENCE_CPP03_ORDER), a->staging.stream(0))
+             : build_on_device(a, a->staging.stream(0));
   }
-  if (rc == NRT_OK) rc = derive_private_layout(a, a->streams[0]);
+  if (rc == NRT_OK) rc = derive_private_layout(a, a->staging.stream(0));
   if (rc != NRT_OK) {
     destroy(a);
     return rc;
@@ -367,23 +293,20 @@ int nrt_adopt(const void *nodes_40B, size_t n_nodes, const uint32_t *indices, si
   if (rc == NRT_OK) rc = upload_geometry(a, verts, stride_bytes, n_verts, faces, n_prims);
   if (rc == NRT_OK) {
     a->n_nodes = n_nodes;
+    cudaStream_t s = a->staging.stream(0);
     cudaError_t e = cudaMalloc(&a->d_nodes, sizeof(Node40) * n_nodes);
     if (e == cudaSuccess) e = cudaMalloc(&a->d_indices, sizeof(uint32_t) * n_indices);
-    if (e == cudaSuccess)
-      e = cudaMemcpyAsync(a->d_nodes, hn, sizeof(Node40) * n_nodes, cudaMemcpyHostToDevice, a->streams[0]);
-    if (e == cudaSuccess)
-      e = cudaMemcpyAsync(a->d_indices, indices, sizeof(uint32_t) * n_indices, cudaMemcpyHostToDevice, a->streams[0]);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(a->streams[0]);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(a->d_nodes, hn, sizeof(Node40) * n_nodes, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(a->d_indices, indices, sizeof(uint32_t) * n_indices, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
     if (e != cudaSuccess) rc = cuda_fail(e, "nrt_adopt upload", __FILE__, __LINE__);
   }
-  if (rc == NRT_OK) rc = derive_private_layout(a, a->streams[0]);
+  if (rc == NRT_OK) rc = derive_private_layout(a, a->staging.stream(0));
   if (rc != NRT_OK) {
     destroy(a);
     return rc;
   }
-  a->h_nodes.assign(hn, hn + n_nodes);
-  a->h_indices.assign(indices, indices + n_indices);
-  a->mirrors_valid = true;
+  a->mirror.assign(hn, n_nodes, indices, n_indices);
   for (int k = 0; k < 3; k++) {
     a->root_bmin[k] = hn[0].bmin[k];
     a->root_bmax[k] = hn[0].bmax[k];
@@ -422,23 +345,12 @@ int nrt_nodes(nrt_accel *h, const void **nodes_40B, size_t *n_nodes, const uint3
     return NRT_ERR_INVALID;
   }
   Accel *a = reinterpret_cast<Accel *>(h);
-  if (!a->mirrors_valid) {
-    NRT_DEVICE(a->device);
-    a->h_nodes.resize(a->n_nodes);
-    a->h_indices.resize(a->n_prims);
-    NRT_CUDA(cudaMemcpy(a->h_nodes.data(), a->d_nodes, sizeof(Node40) * a->n_nodes, cudaMemcpyDeviceToHost));
-    NRT_CUDA(cudaMemcpy(a->h_indices.data(), a->d_indices, sizeof(uint32_t) * a->n_prims, cudaMemcpyDeviceToHost));
-    a->mirrors_valid = true;
-  }
-  if (nodes_40B) *nodes_40B = a->h_nodes.data();
-  if (n_nodes) *n_nodes = a->h_nodes.size();
-  if (indices) *indices = a->h_indices.data();
-  if (n_indices) *n_indices = a->h_indices.size();
-  return NRT_OK;
+  return a->mirror.get(a->device, a->d_nodes, a->n_nodes, a->d_indices, a->n_prims, nodes_40B, n_nodes, indices,
+                       n_indices);
 }
 
 // Any number of calls of one accel may be in flight on any streams: fast launches take their ray cursor from the
-// accel's ring, whose slots are ordered on the device by Accel::ring_done (traverse.cu:launch_fast3_any).
+// accel's ring, whose slots are ordered on the device (traverse.cu:launch_fast3_any).
 int nrt_traverse_device(const nrt_accel *h, const void *d_rays_36B, size_t n_rays, void *d_hits_16B,
                         uint8_t *d_hit_mask, const void *trace_opts_16B, uint32_t flags, void *stream) {
   if (!h || (n_rays && (!d_rays_36B || !d_hits_16B))) {
@@ -496,8 +408,8 @@ int nrt_traverse_lane_stats_device(const nrt_accel *h, const void *d_rays_36B, s
   return NRT_OK;
 }
 
-// Host-pointer path: chunks of rays flow H2D -> traverse -> D2H through three
-// stream slots so that the copy engines (both directions) and the SMs overlap.
+// Host-pointer path: a few rays go through the zero-copy pool (not serialised with other host threads), more through
+// the staging pipeline.  RAY32 calls move 32 B per ray (the pool's slots are laid out for 36 B).
 int nrt_traverse(const nrt_accel *h, const void *rays_36B, size_t n_rays, void *hits_16B, uint8_t *hit_mask,
                  const void *trace_opts_16B, uint32_t flags) {
   if (!h || (n_rays && (!rays_36B || !hits_16B))) {
@@ -508,49 +420,22 @@ int nrt_traverse(const nrt_accel *h, const void *rays_36B, size_t n_rays, void *
   Accel *a = const_cast<Accel *>(reinterpret_cast<const Accel *>(h));
   TraceOptions16 opt = default_trace_options();
   if (trace_opts_16B) memcpy(&opt, trace_opts_16B, sizeof(opt));
-  if (n_rays <= Accel::kSmallRays) {  // low-latency path, not serialised with other host threads
-    NRT_DEVICE(a->device);
-    return traverse_small(a, rays_36B, n_rays, hits_16B, hit_mask, opt, flags);
-  }
-  std::lock_guard<std::mutex> lock(a->host_mu);
+  const size_t ray_bytes = (flags & NRT_TRAVERSE_RAY32) ? 32 : sizeof(Ray36);
   NRT_DEVICE(a->device);
-  const size_t kChunk = (size_t)1 << 20;  // 1 Mi rays = 36 MiB up, 17 MiB down per chunk
-  size_t chunk = std::min(n_rays, kChunk);
-  int rc = ensure_staging(a, std::max(chunk, a->stage_rays));
-  if (rc != NRT_OK) return rc;
-  chunk = std::min(n_rays, a->stage_rays);
-  const char *src = static_cast<const char *>(rays_36B);
-  char *dst = static_cast<char *>(hits_16B);
-  const size_t ray_bytes = (flags & NRT_TRAVERSE_RAY32) ? 32 : sizeof(Ray36);  // the staging slots hold 36 B per ray
-  size_t done = 0;
-  int slot = 0;
-  cudaError_t e = cudaSuccess;
-  while (done < n_rays && rc == NRT_OK && e == cudaSuccess) {
-    size_t m = std::min(chunk, n_rays - done);
-    cudaStream_t s = a->streams[slot];
-    // the slot's previous chunk (3 iterations ago) must have drained before its buffers are reused
-    e = cudaStreamSynchronize(s);
-    if (e == cudaSuccess)
-      e = cudaMemcpyAsync(a->d_stage_rays[slot], src + done * ray_bytes, m * ray_bytes, cudaMemcpyHostToDevice, s);
-    if (e != cudaSuccess) break;
-    rc = launch_traverse(a, static_cast<const Ray36 *>(a->d_stage_rays[slot]), m,
-                         static_cast<Hit16 *>(a->d_stage_hits[slot]),
-                         hit_mask ? static_cast<uint8_t *>(a->d_stage_mask[slot]) : nullptr, opt, flags, s);
-    if (rc != NRT_OK) break;
-    e = cudaMemcpyAsync(dst + done * sizeof(Hit16), a->d_stage_hits[slot], m * sizeof(Hit16), cudaMemcpyDeviceToHost, s);
-    if (e == cudaSuccess && hit_mask)
-      e = cudaMemcpyAsync(hit_mask + done, a->d_stage_mask[slot], m, cudaMemcpyDeviceToHost, s);
-    done += m;
-    slot = (slot + 1) % 3;
+  if (n_rays <= decltype(a->small)::kMaxRays) {
+    return a->small.run(rays_36B, n_rays, ray_bytes, hits_16B, hit_mask,
+                        [&](int i, void *h_rays, void *h_hits, uint8_t *h_mask, cudaStream_t s) {
+                          return launch_traverse(a, static_cast<const Ray36 *>(h_rays), n_rays, static_cast<Hit16 *>(h_hits),
+                                                 h_mask, opt, flags, s,
+                                                 reinterpret_cast<unsigned long long *>(a->d_counters) +
+                                                     Accel::kSmallCursor0 + i);
+                        });
   }
-  // success or not, nothing may still be writing into the caller's buffers when this call returns
-  for (int i = 0; i < 3; i++) {
-    const cudaError_t es = cudaStreamSynchronize(a->streams[i]);
-    if (e == cudaSuccess) e = es;
-  }
-  if (rc != NRT_OK) return rc;
-  NRT_CUDA(e);
-  return NRT_OK;
+  return a->staging.run(rays_36B, n_rays, ray_bytes, hits_16B, sizeof(Hit16), hit_mask,
+                        [&](const void *d_rays, size_t m, void *d_hits, uint8_t *d_mask, cudaStream_t s) {
+                          return launch_traverse(a, static_cast<const Ray36 *>(d_rays), m, static_cast<Hit16 *>(d_hits),
+                                                 d_mask, opt, flags, s);
+                        });
 }
 
 void *nrt_host_alloc(size_t bytes) {

@@ -1472,7 +1472,7 @@ int build_on_device(Accel *a, cudaStream_t s) {
     a->stats.num_leaf_nodes = hc.n_leaves;
     a->stats.num_branch_nodes = n_nodes - hc.n_leaves;
     a->stats.build_secs = ms * 1e-3f;
-    a->mirrors_valid = false;
+    a->mirror.invalidate();
   }
 
 done:

@@ -773,7 +773,7 @@ int build_reference_tree_on_device(Accel *a, bool cpp11_order, cudaStream_t s) {
                                              o.min_leaf_primitives, o.max_tree_depth, o.shallow_depth,
                                              o.min_primitives_for_parallel_build, cpp11_order, &a->d_nodes,
                                              &a->d_indices, &a->n_nodes, &a->stats, a->root_bmin, a->root_bmax, s);
-  if (rc == NRT_OK) a->mirrors_valid = false;
+  if (rc == NRT_OK) a->mirror.invalidate();
   return rc;
 }
 

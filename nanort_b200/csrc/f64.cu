@@ -18,7 +18,6 @@
 #include <math_constants.h>
 
 #include <algorithm>
-#include <condition_variable>
 #include <cstring>
 #include <new>
 #include <vector>
@@ -56,36 +55,19 @@ struct AccelF64 {
   double *d_verts = nullptr;  // packed xyz
   BuildStats16 stats;
   double root_bmin[3], root_bmax[3];
-  std::vector<Node64> h_nodes;
-  std::vector<uint32_t> h_indices;
-  bool mirrors_valid = false;
-  cudaStream_t stream = nullptr;
-  // Traverse: three staging slots, each with its own stream (copy up / traverse / copy down overlap across chunks)
-  cudaStream_t tstream[3] = {nullptr, nullptr, nullptr};
-  void *d_rays[3] = {nullptr, nullptr, nullptr}, *d_hits[3] = {nullptr, nullptr, nullptr}, *d_mask[3] = {nullptr, nullptr, nullptr};
-  size_t stage = 0;
-  // fast-path layout (f64_fast.cuh), derived on the first fast Traverse
+  HostMirror<Node64> mirror;
+  cudaStream_t stream = nullptr;  // build and layout kernels
+  StagingPipeline staging;        // nrt_traverse_f64
+  // fast-path layout (f64_fast.cuh), derived on the first fast Traverse; mu guards the derivation
   void *d_pair = nullptr, *d_tris_fast = nullptr;
-  // ring of 8 ray-pool cursors: cursor_done[k] is recorded after the last launch that used cursor k, and the next
-  // launch on cursor k makes its stream wait for it, so any number of launches in flight never share a cursor.
-  // cursor_next and the events are guarded by mu.
-  static constexpr unsigned kCursors = 8;
-  unsigned long long *d_cursor = nullptr;
-  unsigned cursor_next = 0;
-  cudaEvent_t cursor_done[kCursors] = {};
   bool fast_ready = false;
   std::mutex mu;
-  // small reference-order calls (the facade's one-ray Traverse): zero-copy slots as in Accel::SmallSlot
-  static constexpr int kSmallSlots = 8;
-  static constexpr size_t kSmallRays = 64;
-  struct SmallSlot {
-    void *h = nullptr;  // rays (kSmallRays x 72 B) | records (x 32 B) | flags (x 1 B)
-    cudaStream_t s = nullptr;
-    bool busy = false;
-  };
-  SmallSlot small[kSmallSlots];
-  std::mutex small_mu;
-  std::condition_variable small_cv;
+  // persistent fast launches take the ray cursor d_cursor[k] of the ring's slot k
+  static constexpr uint32_t kCursors = 8;
+  unsigned long long *d_cursor = nullptr;
+  LaunchRing<kCursors> ring;
+  // nrt_traverse_f64 of <= 64 rays in the reference's order (the facade's one-ray Traverse)
+  SmallCallPool<8, sizeof(Ray72), sizeof(Hit32)> small;
 };
 
 void destroy_f64(AccelF64 *a) {
@@ -95,23 +77,29 @@ void destroy_f64(AccelF64 *a) {
   cudaFree(a->d_indices);
   cudaFree(a->d_faces);
   cudaFree(a->d_verts);
-  for (int i = 0; i < 3; i++) {
-    cudaFree(a->d_rays[i]);
-    cudaFree(a->d_hits[i]);
-    cudaFree(a->d_mask[i]);
-    if (a->tstream[i]) cudaStreamDestroy(a->tstream[i]);
-  }
-  for (int i = 0; i < AccelF64::kSmallSlots; i++) {
-    if (a->small[i].h) cudaFreeHost(a->small[i].h);
-    if (a->small[i].s) cudaStreamDestroy(a->small[i].s);
-  }
   cudaFree(a->d_pair);
   cudaFree(a->d_tris_fast);
   cudaFree(a->d_cursor);
-  for (cudaEvent_t e : a->cursor_done)
-    if (e) cudaEventDestroy(e);
   if (a->stream) cudaStreamDestroy(a->stream);
   delete a;
+}
+
+// Packs the (strided) double vertices and uploads them and the faces on a new build stream a->stream (non-blocking,
+// so the copies are stream-ordered with the kernels that consume them, see api.cu:upload_geometry).
+int upload_geometry_f64(AccelF64 *a, const double *verts, size_t stride_bytes, const uint32_t *faces) {
+  const size_t nv = a->n_verts;
+  std::vector<double> packed(3 * nv);
+  for (size_t i = 0; i < nv; i++) {
+    const double *p = reinterpret_cast<const double *>(reinterpret_cast<const char *>(verts) + i * stride_bytes);
+    packed[3 * i] = p[0], packed[3 * i + 1] = p[1], packed[3 * i + 2] = p[2];
+  }
+  NRT_CUDA(cudaStreamCreateWithFlags(&a->stream, cudaStreamNonBlocking));
+  NRT_CUDA(cudaMalloc(&a->d_verts, sizeof(double) * 3 * nv));
+  NRT_CUDA(cudaMalloc(&a->d_faces, sizeof(uint32_t) * 3 * (size_t)a->n_prims));
+  NRT_CUDA(cudaMemcpyAsync(a->d_verts, packed.data(), sizeof(double) * 3 * nv, cudaMemcpyHostToDevice, a->stream));
+  NRT_CUDA(cudaMemcpyAsync(a->d_faces, faces, sizeof(uint32_t) * 3 * (size_t)a->n_prims, cudaMemcpyHostToDevice, a->stream));
+  NRT_CUDA(cudaStreamSynchronize(a->stream));
+  return NRT_OK;
 }
 
 // ---- build ---------------------------------------------------------------------------------------------------
@@ -235,8 +223,9 @@ __global__ void __launch_bounds__(128)
 #include "f64_fast.cuh"
 
 // PairNodeD / TriD arrays of the fast kernel from the BVHNode<double> array, indices_, faces and double vertices the
-// accel already holds on the device.  Called under a->mu.
+// accel already holds on the device, on the first call.
 int derive_fast_layout_f64(AccelF64 *a) {
+  std::lock_guard<std::mutex> lock(a->mu);
   if (a->fast_ready) return NRT_OK;
   const uint32_t nn = (uint32_t)a->n_nodes;
   uint32_t *d_flags = nullptr, *d_widx = nullptr;
@@ -275,28 +264,35 @@ int derive_fast_layout_f64(AccelF64 *a) {
   return NRT_OK;
 }
 
-// Called under a->mu, which orders taking the cursor, waiting for its previous launch, zeroing it, launching and
-// recording the same way on the host and on the device.
-template <int DEPTH>
-cudaError_t launch_fast_f64(AccelF64 *a, const Ray72 *d_rays, size_t m, Hit32 *d_hits, uint8_t *d_mask,
-                            const TraceOptions16 &opt, uint32_t flags, cudaStream_t s) {
-  const unsigned k = a->cursor_next++ % AccelF64::kCursors;
-  unsigned long long *cursor = a->d_cursor + k;
-  cudaEvent_t &done = a->cursor_done[k];
-  cudaError_t e = done ? cudaSuccess : cudaEventCreateWithFlags(&done, cudaEventDisableTiming);
-  if (e == cudaSuccess) e = cudaStreamWaitEvent(s, done, 0);
-  if (e == cudaSuccess) e = cudaMemsetAsync(cursor, 0, sizeof(unsigned long long), s);
-  if (e != cudaSuccess) return e;
+// One launch over m rays on `s`: the reference-order walk, or the fast kernel (its layout derived beforehand) with the
+// ray cursor of the next slot of the accel's ring.
+int launch_f64(AccelF64 *a, const Ray72 *d_rays, size_t m, Hit32 *d_hits, uint8_t *d_mask, const TraceOptions16 &opt,
+               uint32_t flags, cudaStream_t s) {
+  if (flags & NRT_TRAVERSE_CONFORMANCE) {
+    traverse_f64_kernel<<<(unsigned)((m + 127) / 128), 128, 0, s>>>(a->d_nodes, a->d_indices, a->d_faces, a->d_verts,
+                                                                     d_rays, m, d_hits, d_mask, opt, flags);
+    NRT_CUDA(cudaGetLastError());
+    return NRT_OK;
+  }
   size_t grid = (size_t)device_sm_count(a->device) * kFastBlocksPerSmD;  // persistent: every SM holds its complement
   const size_t need = ((m + 31) / 32 + kFastBlockD / 32 - 1) / (kFastBlockD / 32);
   if (grid > need) grid = need;
   if (grid == 0) grid = 1;
-  traverse_fast_f64_kernel<DEPTH><<<(unsigned)grid, kFastBlockD, 0, s>>>(
-      static_cast<const PairNodeD *>(a->d_pair), static_cast<const TriD *>(a->d_tris_fast), d_rays, m, d_hits, d_mask, opt,
-      flags, cursor);
-  e = cudaGetLastError();
-  if (e != cudaSuccess) return e;
-  return cudaEventRecord(done, s);
+  const bool deep = a->stats.max_tree_depth + 2 > 64u;  // adopted reference trees reach depth 256
+  const PairNodeD *pair = static_cast<const PairNodeD *>(a->d_pair);
+  const TriD *tris = static_cast<const TriD *>(a->d_tris_fast);
+  return a->ring.run(s, [&](uint32_t k) {
+    unsigned long long *cursor = a->d_cursor + k;
+    NRT_CUDA(cudaMemsetAsync(cursor, 0, sizeof(unsigned long long), s));
+    if (deep)
+      traverse_fast_f64_kernel<512><<<(unsigned)grid, kFastBlockD, 0, s>>>(pair, tris, d_rays, m, d_hits, d_mask, opt, flags,
+                                                                          cursor);
+    else
+      traverse_fast_f64_kernel<64><<<(unsigned)grid, kFastBlockD, 0, s>>>(pair, tris, d_rays, m, d_hits, d_mask, opt, flags,
+                                                                         cursor);
+    NRT_CUDA(cudaGetLastError());
+    return NRT_OK;
+  });
 }
 
 }  // namespace
@@ -356,11 +352,7 @@ int nrt_build_f64_ex(const double *verts, size_t stride_bytes, size_t n_verts, c
   DeviceGuard dg_caller;  // select_device makes the chosen device current; the caller gets its own back
   int rc = select_device(&device);
   if (rc != NRT_OK) return rc;
-  if (n_verts == 0) {
-    uint32_t m = 0;
-    for (size_t k = 0; k < (size_t)n_prims * 3; k++) m = std::max(m, faces[k]);
-    n_verts = (size_t)m + 1;
-  }
+  if (n_verts == 0) n_verts = infer_n_verts(faces, n_prims);
   AccelF64 *a = new (std::nothrow) AccelF64();
   Accel *t = new (std::nothrow) Accel();  // float topology, discarded after the refit
   uint32_t *d_parent = nullptr, *d_arrived = nullptr;
@@ -372,25 +364,10 @@ int nrt_build_f64_ex(const double *verts, size_t stride_bytes, size_t n_verts, c
   a->device = t->device = device;
   a->n_prims = t->n_prims = n_prims;
   a->n_verts = t->n_verts = n_verts;
-  {
-    std::vector<double> packed(3 * n_verts);
-    for (size_t i = 0; i < n_verts; i++) {
-      const double *p = reinterpret_cast<const double *>(reinterpret_cast<const char *>(verts) + i * stride_bytes);
-      packed[3 * i] = p[0], packed[3 * i + 1] = p[1], packed[3 * i + 2] = p[2];
-    }
-    F64_CUDA(cudaStreamCreateWithFlags(&a->stream, cudaStreamNonBlocking));
-    F64_CUDA(cudaMalloc(&a->d_verts, sizeof(double) * 3 * n_verts));
-    F64_CUDA(cudaMalloc(&a->d_faces, sizeof(uint32_t) * 3 * (size_t)n_prims));
-    F64_CUDA(cudaMalloc(&t->d_verts, sizeof(float) * 3 * n_verts));
-    // stream-ordered with the kernels that consume them (a->stream is non-blocking, see api.cu:upload_geometry)
-    F64_CUDA(cudaMemcpyAsync(a->d_verts, packed.data(), sizeof(double) * 3 * n_verts, cudaMemcpyHostToDevice, a->stream));
-    F64_CUDA(cudaMemcpyAsync(a->d_faces, faces, sizeof(uint32_t) * 3 * (size_t)n_prims, cudaMemcpyHostToDevice, a->stream));
-    F64_CUDA(cudaStreamSynchronize(a->stream));
-  }
+  rc = upload_geometry_f64(a, verts, stride_bytes, faces);
+  if (rc != NRT_OK) goto fail;
   if (flags & NRT_BUILD_REFERENCE_TREE) {
     // conformance build: the reference's own BVHNode<double> array and indices_, bit for bit (build_ref.cu)
-    cudaFree(t->d_verts);
-    t->d_verts = nullptr;
     rc = build_reference_tree<double>(a->d_verts, a->d_faces, nullptr, n_prims, o64.bin_size, o64.min_leaf_primitives,
                                       o64.max_tree_depth, o64.shallow_depth, o64.min_primitives_for_parallel_build,
                                       (flags & NRT_BUILD_REFERENCE_CPP03_ORDER) == 0, &a->d_nodes, &a->d_indices,
@@ -408,6 +385,7 @@ int nrt_build_f64_ex(const double *verts, size_t stride_bytes, size_t n_verts, c
   t->options.bin_size = o64.bin_size;
   t->options.shallow_depth = o64.shallow_depth;
   t->options.min_primitives_for_parallel_build = o64.min_primitives_for_parallel_build;
+  F64_CUDA(cudaMalloc(&t->d_verts, sizeof(float) * 3 * n_verts));
   f64_round_kernel<<<(unsigned)((3 * n_verts + 255) / 256), 256, 0, a->stream>>>(a->d_verts, 3 * n_verts, t->d_verts);
   F64_CUDA(cudaGetLastError());
   rc = build_on_device(t, a->stream);
@@ -477,11 +455,7 @@ int nrt_adopt_f64(const void *nodes_64B, size_t n_nodes, const uint32_t *indices
   DeviceGuard dg_caller;  // select_device makes the chosen device current; the caller gets its own back
   int rc = select_device(&device);
   if (rc != NRT_OK) return rc;
-  if (n_verts == 0) {
-    uint32_t m = 0;
-    for (size_t k = 0; k < (size_t)n_prims * 3; k++) m = std::max(m, faces[k]);
-    n_verts = (size_t)m + 1;
-  }
+  if (n_verts == 0) n_verts = infer_n_verts(faces, n_prims);
   AccelF64 *a = new (std::nothrow) AccelF64();
   if (!a) return NRT_ERR_NOMEM;
   a->device = device;
@@ -489,26 +463,17 @@ int nrt_adopt_f64(const void *nodes_64B, size_t n_nodes, const uint32_t *indices
   a->n_verts = n_verts;
   a->n_nodes = n_nodes;
   a->stats = st;
-  std::vector<double> packed(3 * n_verts);
-  for (size_t i = 0; i < n_verts; i++) {
-    const double *p = reinterpret_cast<const double *>(reinterpret_cast<const char *>(verts) + i * stride_bytes);
-    packed[3 * i] = p[0], packed[3 * i + 1] = p[1], packed[3 * i + 2] = p[2];
+  rc = upload_geometry_f64(a, verts, stride_bytes, faces);
+  if (rc == NRT_OK) {
+    cudaError_t e = cudaMalloc(&a->d_nodes, sizeof(Node64) * n_nodes);
+    if (e == cudaSuccess) e = cudaMalloc(&a->d_indices, sizeof(uint32_t) * n_indices);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(a->d_nodes, hn, sizeof(Node64) * n_nodes, cudaMemcpyHostToDevice, a->stream);
+    if (e == cudaSuccess)
+      e = cudaMemcpyAsync(a->d_indices, indices, sizeof(uint32_t) * n_indices, cudaMemcpyHostToDevice, a->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(a->stream);
+    if (e != cudaSuccess) rc = cuda_fail(e, "nrt_adopt_f64 upload", __FILE__, __LINE__);
   }
-  cudaError_t e = cudaStreamCreateWithFlags(&a->stream, cudaStreamNonBlocking);
-  if (e == cudaSuccess) e = cudaMalloc(&a->d_verts, sizeof(double) * 3 * n_verts);
-  if (e == cudaSuccess) e = cudaMalloc(&a->d_faces, sizeof(uint32_t) * 3 * (size_t)n_prims);
-  if (e == cudaSuccess) e = cudaMalloc(&a->d_nodes, sizeof(Node64) * n_nodes);
-  if (e == cudaSuccess) e = cudaMalloc(&a->d_indices, sizeof(uint32_t) * n_indices);
-  if (e == cudaSuccess)
-    e = cudaMemcpyAsync(a->d_verts, packed.data(), sizeof(double) * 3 * n_verts, cudaMemcpyHostToDevice, a->stream);
-  if (e == cudaSuccess)
-    e = cudaMemcpyAsync(a->d_faces, faces, sizeof(uint32_t) * 3 * (size_t)n_prims, cudaMemcpyHostToDevice, a->stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(a->d_nodes, hn, sizeof(Node64) * n_nodes, cudaMemcpyHostToDevice, a->stream);
-  if (e == cudaSuccess)
-    e = cudaMemcpyAsync(a->d_indices, indices, sizeof(uint32_t) * n_indices, cudaMemcpyHostToDevice, a->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(a->stream);
-  if (e != cudaSuccess) {
-    rc = cuda_fail(e, "nrt_adopt_f64 upload", __FILE__, __LINE__);
+  if (rc != NRT_OK) {
     destroy_f64(a);
     return rc;
   }
@@ -516,9 +481,7 @@ int nrt_adopt_f64(const void *nodes_64B, size_t n_nodes, const uint32_t *indices
     a->root_bmin[k] = hn[0].bmin[k];
     a->root_bmax[k] = hn[0].bmax[k];
   }
-  a->h_nodes.assign(hn, hn + n_nodes);
-  a->h_indices.assign(indices, indices + n_indices);
-  a->mirrors_valid = true;
+  a->mirror.assign(hn, n_nodes, indices, n_indices);
   *out = reinterpret_cast<nrt_accel_f64 *>(a);
   return NRT_OK;
 }
@@ -554,20 +517,8 @@ int nrt_nodes_f64(nrt_accel_f64 *h, const void **nodes_64B, size_t *n_nodes, con
     return NRT_ERR_INVALID;
   }
   AccelF64 *a = reinterpret_cast<AccelF64 *>(h);
-  std::lock_guard<std::mutex> lock(a->mu);
-  if (!a->mirrors_valid) {
-    NRT_DEVICE(a->device);
-    a->h_nodes.resize(a->n_nodes);
-    a->h_indices.resize(a->n_prims);
-    NRT_CUDA(cudaMemcpy(a->h_nodes.data(), a->d_nodes, sizeof(Node64) * a->n_nodes, cudaMemcpyDeviceToHost));
-    NRT_CUDA(cudaMemcpy(a->h_indices.data(), a->d_indices, sizeof(uint32_t) * a->n_prims, cudaMemcpyDeviceToHost));
-    a->mirrors_valid = true;
-  }
-  if (nodes_64B) *nodes_64B = a->h_nodes.data();
-  if (n_nodes) *n_nodes = a->h_nodes.size();
-  if (indices) *indices = a->h_indices.data();
-  if (n_indices) *n_indices = a->h_indices.size();
-  return NRT_OK;
+  return a->mirror.get(a->device, a->d_nodes, a->n_nodes, a->d_indices, a->n_prims, nodes_64B, n_nodes, indices,
+                       n_indices);
 }
 
 int nrt_traverse_f64(const nrt_accel_f64 *h, const void *rays_72B, size_t n_rays, void *hits_32B, uint8_t *hit_mask,
@@ -580,109 +531,30 @@ int nrt_traverse_f64(const nrt_accel_f64 *h, const void *rays_72B, size_t n_rays
   AccelF64 *a = const_cast<AccelF64 *>(reinterpret_cast<const AccelF64 *>(h));
   TraceOptions16 opt = default_trace_options();
   if (trace_opts_16B) memcpy(&opt, trace_opts_16B, sizeof(opt));
-  if (n_rays <= AccelF64::kSmallRays && (flags & NRT_TRAVERSE_CONFORMANCE)) {
-    // low-latency path of the facade's per-ray Traverse: the kernel reads the rays from and writes the records to a
-    // pinned host slot (zero copy), one synchronisation, host threads side by side
-    NRT_DEVICE(a->device);
-    const size_t off_hits = AccelF64::kSmallRays * sizeof(Ray72), off_mask = off_hits + AccelF64::kSmallRays * sizeof(Hit32);
-    int idx = -1;
-    {
-      std::unique_lock<std::mutex> lk(a->small_mu);
-      for (;;) {
-        for (int i = 0; i < AccelF64::kSmallSlots && idx < 0; i++)
-          if (!a->small[i].busy) idx = i;
-        if (idx >= 0) break;
-        a->small_cv.wait(lk);
-      }
-      a->small[idx].busy = true;
-    }
-    AccelF64::SmallSlot &sl = a->small[idx];
-    cudaError_t e = cudaSuccess;
-    if (!sl.h) e = cudaHostAlloc(&sl.h, off_mask + AccelF64::kSmallRays, cudaHostAllocPortable | cudaHostAllocMapped);
-    if (e == cudaSuccess && !sl.s) e = cudaStreamCreateWithFlags(&sl.s, cudaStreamNonBlocking);
-    if (e == cudaSuccess) {
-      char *hb = static_cast<char *>(sl.h);
-      memcpy(hb, rays_72B, n_rays * sizeof(Ray72));
-      traverse_f64_kernel<<<1, 64, 0, sl.s>>>(a->d_nodes, a->d_indices, a->d_faces, a->d_verts,
-                                             reinterpret_cast<const Ray72 *>(hb), n_rays, reinterpret_cast<Hit32 *>(hb + off_hits),
-                                             hit_mask ? reinterpret_cast<uint8_t *>(hb + off_mask) : nullptr, opt, flags);
-      e = cudaGetLastError();
-      const cudaError_t es = cudaStreamSynchronize(sl.s);
-      if (e == cudaSuccess) e = es;
-      if (e == cudaSuccess) {
-        memcpy(hits_32B, hb + off_hits, n_rays * sizeof(Hit32));
-        if (hit_mask) memcpy(hit_mask, hb + off_mask, n_rays);
-      }
-    }
-    {
-      std::lock_guard<std::mutex> lk(a->small_mu);
-      sl.busy = false;
-    }
-    a->small_cv.notify_one();
-    NRT_CUDA(e);
-    return NRT_OK;
-  }
-  std::lock_guard<std::mutex> lock(a->mu);  // Traverse is const and thread-safe in the reference; staging is shared
   NRT_DEVICE(a->device);
-  const bool fast = (flags & NRT_TRAVERSE_CONFORMANCE) == 0;
-  if (fast) {
+  if (n_rays <= decltype(a->small)::kMaxRays && (flags & NRT_TRAVERSE_CONFORMANCE)) {
+    // low-latency path of the facade's per-ray Traverse
+    return a->small.run(rays_72B, n_rays, sizeof(Ray72), hits_32B, hit_mask,
+                        [&](int, void *h_rays, void *h_hits, uint8_t *h_mask, cudaStream_t s) {
+                          traverse_f64_kernel<<<1, 64, 0, s>>>(a->d_nodes, a->d_indices, a->d_faces, a->d_verts,
+                                                               static_cast<const Ray72 *>(h_rays), n_rays,
+                                                               static_cast<Hit32 *>(h_hits), h_mask, opt, flags);
+                          NRT_CUDA(cudaGetLastError());
+                          return NRT_OK;
+                        });
+  }
+  if (!(flags & NRT_TRAVERSE_CONFORMANCE)) {
     const int rc = derive_fast_layout_f64(a);
     if (rc != NRT_OK) return rc;
   }
-  const size_t chunk = std::min(n_rays, (size_t)1 << 20);  // 1 Mi rays = 72 MiB up, 33 MiB down per chunk
-  if (a->stage < chunk) {
-    for (int i = 0; i < 3; i++) {
-      cudaFree(a->d_rays[i]);
-      cudaFree(a->d_hits[i]);
-      cudaFree(a->d_mask[i]);
-      a->d_rays[i] = a->d_hits[i] = a->d_mask[i] = nullptr;
-    }
-    a->stage = 0;
-    for (int i = 0; i < 3; i++) {
-      if (!a->tstream[i]) NRT_CUDA(cudaStreamCreateWithFlags(&a->tstream[i], cudaStreamNonBlocking));
-      NRT_CUDA(cudaMalloc(&a->d_rays[i], chunk * sizeof(Ray72)));
-      NRT_CUDA(cudaMalloc(&a->d_hits[i], chunk * sizeof(Hit32)));
-      NRT_CUDA(cudaMalloc(&a->d_mask[i], chunk));
-    }
-    a->stage = chunk;
-  }
-  const char *src = static_cast<const char *>(rays_72B);
-  char *dst = static_cast<char *>(hits_32B);
-  const bool deep = a->stats.max_tree_depth + 2 > 64u;  // adopted reference trees reach depth 256
-  cudaError_t e = cudaSuccess;
-  int slot = 0;
-  for (size_t done = 0; done < n_rays && e == cudaSuccess; done += chunk) {
-    const size_t m = std::min(chunk, n_rays - done);
-    cudaStream_t s = a->tstream[slot];
-    e = cudaStreamSynchronize(s);  // the slot's previous chunk (3 iterations ago) has drained
-    if (e == cudaSuccess)
-      e = cudaMemcpyAsync(a->d_rays[slot], src + done * sizeof(Ray72), m * sizeof(Ray72), cudaMemcpyHostToDevice, s);
-    if (e != cudaSuccess) break;
-    const Ray72 *d_r = static_cast<const Ray72 *>(a->d_rays[slot]);
-    Hit32 *d_h = static_cast<Hit32 *>(a->d_hits[slot]);
-    uint8_t *d_m = static_cast<uint8_t *>(a->d_mask[slot]);
-    if (fast) {
-      e = deep ? launch_fast_f64<512>(a, d_r, m, d_h, d_m, opt, flags, s) : launch_fast_f64<64>(a, d_r, m, d_h, d_m, opt, flags, s);
-    } else {
-      traverse_f64_kernel<<<(unsigned)((m + 127) / 128), 128, 0, s>>>(a->d_nodes, a->d_indices, a->d_faces, a->d_verts, d_r,
-                                                                      m, d_h, d_m, opt, flags);
-      e = cudaGetLastError();
-    }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(dst + done * sizeof(Hit32), d_h, m * sizeof(Hit32), cudaMemcpyDeviceToHost, s);
-    if (e == cudaSuccess && hit_mask) e = cudaMemcpyAsync(hit_mask + done, d_m, m, cudaMemcpyDeviceToHost, s);
-    slot = (slot + 1) % 3;
-  }
-  // success or not, nothing may still be writing into the caller's buffers when this call returns
-  for (int i = 0; i < 3; i++) {
-    const cudaError_t es = a->tstream[i] ? cudaStreamSynchronize(a->tstream[i]) : cudaSuccess;
-    if (e == cudaSuccess) e = es;
-  }
-  NRT_CUDA(e);
-  return NRT_OK;
+  return a->staging.run(rays_72B, n_rays, sizeof(Ray72), hits_32B, sizeof(Hit32), hit_mask,
+                        [&](const void *d_rays, size_t m, void *d_hits, uint8_t *d_mask, cudaStream_t s) {
+                          return launch_f64(a, static_cast<const Ray72 *>(d_rays), m, static_cast<Hit32 *>(d_hits),
+                                            d_mask, opt, flags, s);
+                        });
 }
 
-// Any number of calls of one accel may be in flight on any streams (launch_fast_f64 orders the cursor ring's slots
-// on the device).
+// Any number of calls of one accel may be in flight on any streams (launch_f64 orders the ring's slots on the device).
 int nrt_traverse_f64_device(const nrt_accel_f64 *h, const void *d_rays_72B, size_t n_rays, void *d_hits_32B,
                             uint8_t *d_hit_mask, const void *trace_opts_16B, uint32_t flags, void *stream) {
   if (!h || (n_rays && (!d_rays_72B || !d_hits_32B))) {
@@ -693,24 +565,13 @@ int nrt_traverse_f64_device(const nrt_accel_f64 *h, const void *d_rays_72B, size
   AccelF64 *a = const_cast<AccelF64 *>(reinterpret_cast<const AccelF64 *>(h));
   TraceOptions16 opt = default_trace_options();
   if (trace_opts_16B) memcpy(&opt, trace_opts_16B, sizeof(opt));
-  std::lock_guard<std::mutex> lock(a->mu);  // lazy layout + the cursor ring (launch_fast_f64)
   NRT_DEVICE(a->device);
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const Ray72 *d_r = static_cast<const Ray72 *>(d_rays_72B);
-  Hit32 *d_h = static_cast<Hit32 *>(d_hits_32B);
-  cudaError_t e;
-  if (flags & NRT_TRAVERSE_CONFORMANCE) {
-    traverse_f64_kernel<<<(unsigned)((n_rays + 127) / 128), 128, 0, s>>>(a->d_nodes, a->d_indices, a->d_faces, a->d_verts, d_r,
-                                                                         n_rays, d_h, d_hit_mask, opt, flags);
-    e = cudaGetLastError();
-  } else {
+  if (!(flags & NRT_TRAVERSE_CONFORMANCE)) {
     const int rc = derive_fast_layout_f64(a);
     if (rc != NRT_OK) return rc;
-    e = a->stats.max_tree_depth + 2 > 64u ? launch_fast_f64<512>(a, d_r, n_rays, d_h, d_hit_mask, opt, flags, s)
-                                          : launch_fast_f64<64>(a, d_r, n_rays, d_h, d_hit_mask, opt, flags, s);
   }
-  NRT_CUDA(e);
-  return NRT_OK;
+  return launch_f64(a, static_cast<const Ray72 *>(d_rays_72B), n_rays, static_cast<Hit32 *>(d_hits_32B), d_hit_mask, opt,
+                    flags, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -268,10 +268,9 @@ int nrt_build_prims(uint32_t kind, const float *data, size_t stride_bytes, const
     set_error("nrt_build_prims: bin_size must be > 1 and max_tree_depth <= 500");
     return fail(NRT_ERR_INVALID);
   }
-  e = cudaMalloc(&a->d_counters, 96 * sizeof(uint64_t));
-  if (e == cudaSuccess) e = cudaMemset(a->d_counters, 0, 96 * sizeof(uint64_t));
-  for (int i = 0; i < 3 && e == cudaSuccess; i++) e = cudaStreamCreateWithFlags(&a->streams[i], cudaStreamNonBlocking);
-  cudaStream_t s = a->streams[0];
+  rc = common_init(a);
+  if (rc != NRT_OK) return fail(rc);
+  cudaStream_t s = a->staging.stream(0);
   if (e == cudaSuccess) e = cudaMalloc(&a->d_prim_boxes, sizeof(float) * 6 * (size_t)n_prims);
   if (kind == NRT_PRIM_SPHERES) {
     const size_t in_bytes = (size_t)(n_prims - 1) * stride_bytes + 12;
@@ -320,7 +319,7 @@ int nrt_list_node_intersections(const nrt_accel *h, const void *rays_36B, size_t
   if (n_rays == 0) return NRT_OK;
   NRT_DEVICE(a->device);
   std::lock_guard<std::mutex> lock(const_cast<Accel *>(a)->host_mu);
-  cudaStream_t s = a->streams[0];
+  cudaStream_t s = a->staging.stream(0);
   Ray36 *d_rays = nullptr;
   NodeHit12 *d_hits = nullptr;
   uint32_t *d_cnt = nullptr;

@@ -602,20 +602,15 @@ struct Scene {
   InstanceDev *d_inst = nullptr;
   float *d_state = nullptr;  // 76 floats per instance
   uint32_t max_blas_depth = 0;
-  // per-launch scratch, handed out round-robin: slot k owns the ray cursor d_counters[k], the overflow count
-  // d_counters[4 + k] and its own overflow list.  slot_done[k] is recorded after the last launch that used slot k,
-  // and the next launch on slot k makes its stream wait for it, so launches in flight on any number of streams never
-  // share a cursor or an overflow list.  next_slot and the events are guarded by mu.
+  // per-launch scratch of the ring's slot k: the ray cursor d_counters[k], the overflow count d_counters[4 + k] and its
+  // own overflow list
   static constexpr int kSlots = 4;
   uint32_t *d_overflow[kSlots] = {nullptr, nullptr, nullptr, nullptr};
   size_t overflow_cap[kSlots] = {0, 0, 0, 0};
-  cudaEvent_t slot_done[kSlots] = {nullptr, nullptr, nullptr, nullptr};
   unsigned long long *d_counters = nullptr;
-  uint32_t next_slot = 0;
-  cudaStream_t stream = nullptr;
-  void *d_rays = nullptr, *d_hits = nullptr, *d_mask = nullptr;
-  size_t stage = 0;
-  std::mutex mu;
+  LaunchRing<kSlots> ring;
+  cudaStream_t stream = nullptr;  // commit
+  StagingPipeline staging;        // nrt_scene_traverse
 };
 
 static void scene_destroy(Scene *s) {
@@ -631,14 +626,8 @@ static void scene_destroy(Scene *s) {
   }
   cudaFree(s->d_inst);
   cudaFree(s->d_state);
-  for (int k = 0; k < Scene::kSlots; k++) {
-    cudaFree(s->d_overflow[k]);
-    if (s->slot_done[k]) cudaEventDestroy(s->slot_done[k]);
-  }
+  for (int k = 0; k < Scene::kSlots; k++) cudaFree(s->d_overflow[k]);
   cudaFree(s->d_counters);
-  cudaFree(s->d_rays);
-  cudaFree(s->d_hits);
-  cudaFree(s->d_mask);
   if (s->stream) cudaStreamDestroy(s->stream);
   delete s;
 }
@@ -664,40 +653,36 @@ static int scene_launch(Scene *sc, const Ray36 *d_rays, size_t n, SceneHit32 *d_
     set_error("nrt_scene_traverse: flags bits 8..15 are reserved");
     return NRT_ERR_INVALID;
   }
-  // the whole launch sequence under the lock: taking the slot, waiting for its previous user, enqueueing the kernels
-  // and recording slot_done happen in the same order on the host and on the device
-  std::lock_guard<std::mutex> lock(sc->mu);
-  const int slot = (int)sc->next_slot;
-  sc->next_slot = (sc->next_slot + 1) % (uint32_t)Scene::kSlots;
-  if (sc->overflow_cap[slot] < n) {  // grows rarely; the launch that last used the old list must be done with it
-    NRT_CUDA(cudaEventSynchronize(sc->slot_done[slot]));
-    cudaFree(sc->d_overflow[slot]);
-    sc->d_overflow[slot] = nullptr;
-    sc->overflow_cap[slot] = 0;
-    NRT_CUDA(cudaMalloc(&sc->d_overflow[slot], sizeof(uint32_t) * n));
-    sc->overflow_cap[slot] = n;
-  }
-  uint32_t *d_overflow = sc->d_overflow[slot];
-  NRT_CUDA(cudaStreamWaitEvent(s, sc->slot_done[slot], 0));
-  unsigned long long *cursor = sc->d_counters + slot;
-  unsigned long long *ovf = sc->d_counters + Scene::kSlots + slot;
-  NRT_CUDA(cudaMemsetAsync(cursor, 0, sizeof(unsigned long long), s));
-  NRT_CUDA(cudaMemsetAsync(ovf, 0, sizeof(unsigned long long), s));
-  const size_t need = ((n + 31) / 32 + 3) / 4;
-  size_t grid = (size_t)sms * (stack_need > 64 ? 2 : kUnifiedMinBlocks);
-  if (grid > need) grid = need;
-  if (stack_need > 64)
-    scene_unified_kernel<1024, 2><<<(unsigned)grid, kSceneBlock, 0, s>>>(dev, d_rays, n, d_hits, d_mask, flags, cursor,
-                                                                      d_overflow, ovf);
-  else
-    scene_unified_kernel<64, kUnifiedMinBlocks><<<(unsigned)grid, kSceneBlock, 0, s>>>(
-        dev, d_rays, n, d_hits, d_mask, flags, cursor, d_overflow, ovf);
-  NRT_CUDA(cudaGetLastError());
-  scene_list_kernel<<<(unsigned)std::min<size_t>((n + 127) / 128, (size_t)sms * 4), 128, 0, s>>>(
-      dev, d_rays, n, d_overflow, ovf, d_hits, d_mask, flags);
-  NRT_CUDA(cudaGetLastError());
-  NRT_CUDA(cudaEventRecord(sc->slot_done[slot], s));
-  return NRT_OK;
+  return sc->ring.run(s, [&](uint32_t slot) {
+    if (sc->overflow_cap[slot] < n) {  // grows rarely; the launch that last used the old list must be done with it
+      const int rc = sc->ring.wait_host(slot);
+      if (rc != NRT_OK) return rc;
+      cudaFree(sc->d_overflow[slot]);
+      sc->d_overflow[slot] = nullptr;
+      sc->overflow_cap[slot] = 0;
+      NRT_CUDA(cudaMalloc(&sc->d_overflow[slot], sizeof(uint32_t) * n));
+      sc->overflow_cap[slot] = n;
+    }
+    uint32_t *d_overflow = sc->d_overflow[slot];
+    unsigned long long *cursor = sc->d_counters + slot;
+    unsigned long long *ovf = sc->d_counters + Scene::kSlots + slot;
+    NRT_CUDA(cudaMemsetAsync(cursor, 0, sizeof(unsigned long long), s));
+    NRT_CUDA(cudaMemsetAsync(ovf, 0, sizeof(unsigned long long), s));
+    const size_t need = ((n + 31) / 32 + 3) / 4;
+    size_t grid = (size_t)sms * (stack_need > 64 ? 2 : kUnifiedMinBlocks);
+    if (grid > need) grid = need;
+    if (stack_need > 64)
+      scene_unified_kernel<1024, 2><<<(unsigned)grid, kSceneBlock, 0, s>>>(dev, d_rays, n, d_hits, d_mask, flags, cursor,
+                                                                        d_overflow, ovf);
+    else
+      scene_unified_kernel<64, kUnifiedMinBlocks><<<(unsigned)grid, kSceneBlock, 0, s>>>(
+          dev, d_rays, n, d_hits, d_mask, flags, cursor, d_overflow, ovf);
+    NRT_CUDA(cudaGetLastError());
+    scene_list_kernel<<<(unsigned)std::min<size_t>((n + 127) / 128, (size_t)sms * 4), 128, 0, s>>>(
+        dev, d_rays, n, d_overflow, ovf, d_hits, d_mask, flags);
+    NRT_CUDA(cudaGetLastError());
+    return NRT_OK;
+  });
 }
 
 }  // namespace nrt
@@ -743,8 +728,6 @@ int nrt_scene_commit(const nrt_instance *instances, uint32_t n_instances, uint32
   if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&sc->stream, cudaStreamNonBlocking);
   if (e == cudaSuccess) e = cudaMalloc(&sc->d_counters, 32 * sizeof(unsigned long long));
   if (e == cudaSuccess) e = cudaMemset(sc->d_counters, 0, 32 * sizeof(unsigned long long));
-  for (int k = 0; k < Scene::kSlots && e == cudaSuccess; k++)
-    e = cudaEventCreateWithFlags(&sc->slot_done[k], cudaEventDisableTiming);
   if (e == cudaSuccess) e = cudaMalloc(&sc->d_inst, sizeof(InstanceDev) * (size_t)n_instances);
   if (e == cudaSuccess) e = cudaMalloc(&sc->d_state, sizeof(float) * 76 * (size_t)n_instances);
   if (e == cudaSuccess) e = cudaMalloc(&d_in, sizeof(InstanceIn) * (size_t)n_instances);
@@ -818,22 +801,9 @@ int nrt_scene_nodes(nrt_scene *s, const void **nodes_40B, size_t *n_nodes, const
     set_error("nrt_scene_nodes: NULL scene");
     return NRT_ERR_INVALID;
   }
-  Scene *sc = reinterpret_cast<Scene *>(s);
-  Accel *a = sc->top;
-  std::lock_guard<std::mutex> lock(sc->mu);
-  if (!a->mirrors_valid) {
-    NRT_DEVICE(sc->device);
-    a->h_nodes.resize(a->n_nodes);
-    a->h_indices.resize(a->n_prims);
-    NRT_CUDA(cudaMemcpy(a->h_nodes.data(), a->d_nodes, sizeof(Node40) * a->n_nodes, cudaMemcpyDeviceToHost));
-    NRT_CUDA(cudaMemcpy(a->h_indices.data(), a->d_indices, sizeof(uint32_t) * a->n_prims, cudaMemcpyDeviceToHost));
-    a->mirrors_valid = true;
-  }
-  if (nodes_40B) *nodes_40B = a->h_nodes.data();
-  if (n_nodes) *n_nodes = a->h_nodes.size();
-  if (indices) *indices = a->h_indices.data();
-  if (n_indices) *n_indices = a->h_indices.size();
-  return NRT_OK;
+  Accel *a = reinterpret_cast<Scene *>(s)->top;
+  return a->mirror.get(a->device, a->d_nodes, a->n_nodes, a->d_indices, a->n_prims, nodes_40B, n_nodes, indices,
+                       n_indices);
 }
 
 int nrt_scene_instance_state(const nrt_scene *s, uint32_t instance, float out76[76]) {
@@ -870,37 +840,11 @@ int nrt_scene_traverse(const nrt_scene *s, const void *rays_36B, size_t n_rays, 
   if (n_rays == 0) return NRT_OK;
   Scene *sc = const_cast<Scene *>(reinterpret_cast<const Scene *>(s));
   NRT_DEVICE(sc->device);
-  const size_t kChunk = (size_t)1 << 20;
-  const size_t chunk = std::min(n_rays, kChunk);
-  // one caller at a time on the staging buffers (Scene::Traverse is const and thread-safe in the reference)
-  static std::mutex host_mu;
-  std::lock_guard<std::mutex> lock(host_mu);
-  if (sc->stage < chunk) {
-    cudaFree(sc->d_rays);
-    cudaFree(sc->d_hits);
-    cudaFree(sc->d_mask);
-    sc->d_rays = sc->d_hits = sc->d_mask = nullptr;
-    sc->stage = 0;
-    NRT_CUDA(cudaMalloc(&sc->d_rays, chunk * sizeof(Ray36)));
-    NRT_CUDA(cudaMalloc(&sc->d_hits, chunk * sizeof(SceneHit32)));
-    NRT_CUDA(cudaMalloc(&sc->d_mask, chunk));
-    sc->stage = chunk;
-  }
-  const char *src = static_cast<const char *>(rays_36B);
-  char *dst = static_cast<char *>(hits_32B);
-  for (size_t done = 0; done < n_rays; done += chunk) {
-    const size_t m = std::min(chunk, n_rays - done);
-    NRT_CUDA(cudaMemcpyAsync(sc->d_rays, src + done * sizeof(Ray36), m * sizeof(Ray36), cudaMemcpyHostToDevice,
-                             sc->stream));
-    int rc = scene_launch(sc, static_cast<const Ray36 *>(sc->d_rays), m, static_cast<SceneHit32 *>(sc->d_hits),
-                          static_cast<uint8_t *>(sc->d_mask), flags, sc->stream);
-    if (rc != NRT_OK) return rc;
-    NRT_CUDA(cudaMemcpyAsync(dst + done * sizeof(SceneHit32), sc->d_hits, m * sizeof(SceneHit32),
-                             cudaMemcpyDeviceToHost, sc->stream));
-    if (hit_mask) NRT_CUDA(cudaMemcpyAsync(hit_mask + done, sc->d_mask, m, cudaMemcpyDeviceToHost, sc->stream));
-    NRT_CUDA(cudaStreamSynchronize(sc->stream));
-  }
-  return NRT_OK;
+  return sc->staging.run(rays_36B, n_rays, sizeof(Ray36), hits_32B, sizeof(SceneHit32), hit_mask,
+                         [&](const void *d_rays, size_t m, void *d_hits, uint8_t *d_mask, cudaStream_t st) {
+                           return scene_launch(sc, static_cast<const Ray36 *>(d_rays), m, static_cast<SceneHit32 *>(d_hits),
+                                               d_mask, flags, st);
+                         });
 }
 
 }  // extern "C"

@@ -198,7 +198,7 @@ static int launch_fast3_cursor(const Accel *a, Rays rays, size_t n, Epi epi, con
 }
 
 // `cursor`: a cursor the caller owns (the small-call slots: held until their launch has finished), or nullptr for the
-// next one of the accel's ring (Accel::ring_done)
+// next one of the accel's ring (Accel::ring)
 template <class Rays, bool COUNT, class P, class Epi>
 static int launch_fast3_any(const Accel *a, Rays rays, size_t n, Epi epi, const TraceOptions16 &opt, uint32_t flags,
                             unsigned long long *d_counts, const unsigned long long *n_ptr, cudaStream_t s,
@@ -208,18 +208,10 @@ static int launch_fast3_any(const Accel *a, Rays rays, size_t n, Epi epi, const 
     return NRT_ERR_INVALID;
   }
   if (cursor) return launch_fast3_cursor<Rays, COUNT, P>(a, rays, n, epi, opt, flags, d_counts, n_ptr, s, cursor);
-  // taking the slot, waiting for its previous launch, zeroing the cursor, launching and recording happen under one
-  // lock, so they are in the same order on the host and on the device
-  std::lock_guard<std::mutex> lock(a->ring_mu);
-  const uint32_t k = a->cursor_ring++ % Accel::kRingSlots;
-  cudaEvent_t &done = a->ring_done[k];
-  if (!done) NRT_CUDA(cudaEventCreateWithFlags(&done, cudaEventDisableTiming));
-  NRT_CUDA(cudaStreamWaitEvent(s, done, 0));
-  cursor = reinterpret_cast<unsigned long long *>(a->d_counters) + 16 + k;
-  const int rc = launch_fast3_cursor<Rays, COUNT, P>(a, rays, n, epi, opt, flags, d_counts, n_ptr, s, cursor);
-  if (rc != NRT_OK) return rc;
-  NRT_CUDA(cudaEventRecord(done, s));
-  return NRT_OK;
+  return a->ring.run(s, [&](uint32_t k) {
+    return launch_fast3_cursor<Rays, COUNT, P>(a, rays, n, epi, opt, flags, d_counts, n_ptr, s,
+                                               reinterpret_cast<unsigned long long *>(a->d_counters) + 16 + k);
+  });
 }
 
 // the default for coherent launches, with the size cut-off
