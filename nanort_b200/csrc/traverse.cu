@@ -142,11 +142,15 @@ int device_sm_count(int device) {
 // incoherent launches 20 (28 and more lose 10-50 % there).
 //                 MINB REFILL PAIR128 LEAF_AGAIN DEFER NODE_UNROLL
 typedef Policy3<10, 24, true, 8, false, 2> DefaultPolicy;
-// The camera launch runs 9 CTAs per SM (56 registers: its AO-spawn retire step spills at 48) and, like the incoherent
-// launches, three node steps per exit check.  Re-swept on H100 (80GB HBM3, 700 W) over the camera-relative layout and
+// The camera launch over the accel's own arrays runs 9 CTAs per SM (56 registers: its AO-spawn retire step spills at
+// 48) and, like the incoherent launches, three node steps per exit check.  Re-swept on H100 (80GB HBM3, 700 W) over the camera-relative layout and
 // the precomputed face normals: MINB 9/10 x NODE_UNROLL 2/3 all lie within 1 % of each other on the bench headline
 // (10 spills 32 B at 48 registers), so this row stays (DESIGN.md section 10).
 typedef Policy3<9, 32, true, 12, true, 3> CameraPolicy;
+// The packet walk of the camera launch over the camera-relative copies (traverse_packet_kernel): 9 CTAs per SM, 56
+// registers and no spills; 10 (48 registers) spills 16 B and lies within 1 %, 12 (40 registers) is 2 % slower
+// (DESIGN.md section 10).
+typedef PacketPolicy<9> CameraPacketPolicy;
 typedef Policy3<10, 20, false, 12, false, 3> IncoherentPolicy;
 typedef Policy3<9, 32, false, 12, true, 3> IncoherentCameraPolicy;
 // The path tracer's radiance launch: its retire step IS the shading block, which needs more registers than the plain
@@ -301,9 +305,41 @@ static int launch_fused(const Accel *a, Rays rays, size_t n, const unsigned long
   return launch_fast3_any<Rays, false, P>(a, rays, n, epi, opt, flags, nullptr, n_ptr, s);
 }
 
+template <int DEPTH>
+static cudaError_t launch_packet(const Accel *a, CameraRays rays, size_t n, const PrimaryToAoEpilogue &epi,
+                                 const TraceOptions16 &opt, uint32_t flags, unsigned long long *cursor, cudaStream_t s) {
+  const size_t warps_per_block = kTraverseBlock / 32;
+  size_t grid = (size_t)device_sm_count(a->device) * CameraPacketPolicy::kMinBlocks;
+  const size_t need_blocks = ((n + 31) / 32 + warps_per_block - 1) / warps_per_block;
+  if (grid > need_blocks) grid = need_blocks;
+  traverse_packet_kernel<CameraRays, DEPTH, CameraPacketPolicy, PrimaryToAoEpilogue>
+      <<<(unsigned)grid, kTraverseBlock, 0, s>>>(a->d_pair_rel, a->d_tris_rel, rays, n, epi, opt, flags, cursor);
+  return cudaGetLastError();
+}
+
+// the packet walk, with a cursor of the accel's ring (as launch_fast3_any); the caller has made the camera-relative copies
+static int launch_packet_any(const Accel *a, CameraRays rays, size_t n, const PrimaryToAoEpilogue &epi,
+                             const TraceOptions16 &opt, uint32_t flags, cudaStream_t s) {
+  if (!a->d_pair_rel || !a->d_tris_rel) {
+    set_error("traverse: this accel has no camera-relative traversal layout");
+    return NRT_ERR_INVALID;
+  }
+  return a->ring.run(s, [&](uint32_t k) {
+    unsigned long long *cursor = reinterpret_cast<unsigned long long *>(a->d_counters) + 16 + k;
+    NRT_CUDA(cudaMemsetAsync(cursor, 0, sizeof(unsigned long long), s));
+    const cudaError_t e = needs_deep_stack(a) ? launch_packet<512>(a, rays, n, epi, opt, flags, cursor, s)
+                                              : launch_packet<64>(a, rays, n, epi, opt, flags, cursor, s);
+    NRT_CUDA(e);
+    return NRT_OK;
+  });
+}
+
 // Camera rays, generated inside the kernel (no generator kernel, no primary queue).  On the PairNode path they read
 // camera-relative copies of the nodes and triangles while the originals and the copies together stay well inside one
 // half of the L2 (kCameraRelMaxBytes); the caller orders `s` after every earlier pass that may still read the copies.
+// Over the copies, each 8x4-pixel packet walks the tree as one warp (traverse_packet_kernel).  The launches over the
+// accel's own arrays keep the per-lane walk: their trees are the ones too big for the copies, and on the 1 M terrain
+// (PairNodes, 86 MB of nodes and triangles against the 50 MB L2) the pass took 26 % longer with the packet walk.
 int launch_traverse_camera_fused(Accel *a, const Wave &w, const nrt_ao_params &p, unsigned long long slot0, size_t count,
                                  const float4 *d_face_n, float *d_accum, unsigned long long *d_wave_counters,
                                  const TraceOptions16 &opt, uint32_t flags, cudaStream_t s) {
@@ -317,7 +353,7 @@ int launch_traverse_camera_fused(Accel *a, const Wave &w, const nrt_ao_params &p
                                                                 nullptr, s);
   const int rc = camera_relative_layout(a, p.cam, s);
   if (rc != NRT_OK) return rc;
-  return launch_fast3_any<CameraRays, false, CameraPolicy>(a, CameraRays(p, slot0), count, epi, opt, flags, nullptr, nullptr, s);
+  return launch_packet_any(a, CameraRays(p, slot0), count, epi, opt, flags, s);
 }
 
 int launch_traverse_ao_fused(const Accel *a, const Wave &w, const unsigned long long *d_count, size_t capacity,

@@ -448,4 +448,150 @@ __global__ void __launch_bounds__(kTraverseBlock, P::kMinBlocks)
   }
 }
 
+// Launch policy of traverse_packet_kernel: a warp always takes a whole packet and retires it whole, so refill, deferred
+// retire, leaf batching and node-step unrolling have nothing to tune
+template <int MINB_>
+struct PacketPolicy {
+  static constexpr int kMinBlocks = MINB_;  // CTAs per SM (the register budget) and of the persistent grid
+};
+
+// Packet traversal for camera rays: the 32 rays a warp takes (32 consecutive slots, one 8x4-pixel block at one sample)
+// walk the tree together.  The node the warp stands on is warp-uniform, and so is the stack pointer: every lane writes
+// and reads its stack at the same index, so stack traffic is coalesced, and no lane postpones a leaf or waits in a
+// vote on the others' phase.  Each lane still runs slab_pair / tri_test3 with its own best.t, enters a child only if
+// its own test accepts it, and skips a popped entry that lies behind its own best (nanort.h:2532) -- only the order of
+// the visits is the warp's (the near child is the one most lanes that hit both children see nearer), the freedom the
+// while-while kernel uses too.
+//
+// A lane that is not entering the current node ("inactive" there) only follows the warp: it runs the node step's loads
+// and slab test with the others, but its hits are dropped (a slot past the end of the ray set has a zeroed ray context
+// whose plane offsets stay inside the node).  The entry distance a lane
+// pushes for a child it did not hit is a NaN, which fails `entry <= best.t` at the pop: a real entry distance is never
+// NaN, since slab_pair's fmaxf chain ends with min_t and fmaxf drops a NaN operand, and range_has_nan() lanes never
+// become active (their min_t / max_t are the only possible NaN there).
+// DEPTH: capacity of the per-lane stack, as traverse_fast3_kernel (a pair pushes one entry and descends one level).
+template <class Rays, int DEPTH, class P, class Epi>
+__global__ void __launch_bounds__(kTraverseBlock, P::kMinBlocks)
+    traverse_packet_kernel(const void *__restrict__ pair, const TriCM *__restrict__ tris, Rays rays, size_t n, Epi epi,
+                           TraceOptions16 opt, uint32_t flags, unsigned long long *cursor) {
+  constexpr bool kRel = Rays::kSharedOrigin;
+  static_assert(!Epi::kAnyHit, "packet walk: closest hit only");
+  const int lane = threadIdx.x & 31;
+  const bool cpp03 = (flags & NRT_TRAVERSE_CPP03_INVERSE) != 0;
+  const bool filtered = opt.prim_ids_range[0] != 0u || opt.prim_ids_range[1] < 0x7FFFFFFFu ||
+                        opt.skip_prim_id < 0x7FFFFFFFu;
+  const float4 *const pair4 = reinterpret_cast<const float4 *>(pair);  // 8 float4 per PairNode
+  const float4 *const tris4 = reinterpret_cast<const float4 *>(tris);  // 3 float4 per TriCM
+  const uint32_t kNoEntry = 0x7FC00000u;                                // quiet NaN: never <= best.t
+
+  // per-lane stack of (ref, entry distance); the extra entries park what only the retire step reads (max_t, payload)
+  constexpr int PW = Rays::kPayloadWords;
+  uint2 lstk[DEPTH + 1 + (PW + 1) / 2];
+
+  for (;;) {
+    unsigned long long base = 0;
+    if (lane == 0) base = atomicAdd(cursor, 32ull);
+    base = __shfl_sync(FULL_MASK, base, 0);
+    if (base >= (unsigned long long)n) break;
+    const unsigned long long mine = base + (unsigned long long)lane;
+    const bool valid = mine < (unsigned long long)n;
+
+    RayCtx3 c = {};  // a slot past the end keeps these: in-range plane offsets for the node step's loads
+    c.ny = 2u;
+    c.nz = 4u;
+    Best best;
+    best.t = 0.0f;
+    best.u = 0.0f;
+    best.v = 0.0f;
+    best.prim = 0xFFFFFFFFu;
+    float min_t = 0.0f;
+    bool active = false;
+    if (valid) {
+      float ox, oy, oz, dx, dy, dz, max_t;
+      uint32_t payload[PW > 0 ? PW : 1];
+      rays.load((size_t)mine, ox, oy, oz, dx, dy, dz, min_t, max_t, payload);
+#pragma unroll
+      for (int w = 0; w + 1 < PW; w += 2) lstk[DEPTH + 1 + w / 2] = make_uint2(payload[w], payload[w + 1]);
+      if (PW & 1) lstk[DEPTH + 1 + PW / 2].x = payload[PW - 1];
+      setup_ray3(c, ox, oy, oz, dx, dy, dz, min_t, cpp03);
+      best.t = max_t;
+      lstk[DEPTH].x = __float_as_uint(max_t);
+      active = !range_has_nan(min_t, max_t);
+    }
+
+    int cur = __any_sync(FULL_MASK, active) ? 0 : kNone3;  // warp-uniform from here on
+    int sp = 0;
+    while (cur != kNone3) {
+      if (cur >= 0) {
+        // every lane tests the pair (no branch around it: the step is issue bound), only active lanes' hits count
+        bool h0, h1;
+        float t0, t1;
+        const uint32_t n8 = (uint32_t)cur * 8u;
+        const int2 R = __ldg(reinterpret_cast<const int2 *>(pair4 + (n8 + 6u)));
+        const float4 X = __ldg(pair4 + (n8 + c.nx));
+        const float4 Y = __ldg(pair4 + (n8 + c.ny));
+        const float4 Z = __ldg(pair4 + (n8 + c.nz));
+        slab_pair<kRel>(c, X, Y, Z, min_t, best.t, h0, h1, t0, t1);
+        h0 &= active;
+        h1 &= active;
+        const unsigned m0 = __ballot_sync(FULL_MASK, h0), m1 = __ballot_sync(FULL_MASK, h1);
+        if (m0 != 0u && m1 != 0u) {
+          // both children are wanted: the one that most lanes hitting both see nearer goes first (the first child when
+          // no lane hits both)
+          const unsigned first1 = __ballot_sync(FULL_MASK, h0 & h1 & (t1 < t0));
+          const bool one = 2 * __popc(first1) > __popc(m0 & m1);
+          lstk[sp] = make_uint2((uint32_t)(one ? R.x : R.y), (one ? h0 : h1) ? __float_as_uint(one ? t0 : t1) : kNoEntry);
+          sp++;
+          cur = one ? R.y : R.x;
+          active = one ? h1 : h0;
+        } else if (m0 != 0u) {
+          cur = R.x;
+          active = h0;
+        } else if (m1 != 0u) {
+          cur = R.y;
+          active = h1;
+        } else {
+          cur = kNone3;
+        }
+      } else {
+        if (active) {
+          uint32_t slot = (uint32_t)(~cur);
+          for (;;) {
+            const uint32_t s3 = slot * 3u;
+            const float4 VX = __ldg(tris4 + (s3 + c.tx));
+            const float4 VY = __ldg(tris4 + (s3 + c.ty));
+            const float4 VZ = __ldg(tris4 + (s3 + c.tz));
+            tri_test3<kRel>(c, opt, filtered, VX, VY, VZ, best);
+            if ((int)__float_as_uint(VX.w) < 0) break;  // last triangle of the leaf
+            slot++;
+          }
+        }
+        cur = kNone3;
+      }
+      // pop until some lane enters the popped entry
+      while (cur == kNone3 && sp > 0) {
+        --sp;
+        const uint2 e = lstk[sp];
+        active = __uint_as_float(e.y) <= best.t;
+        if (__any_sync(FULL_MASK, active)) cur = (int)e.x;
+      }
+    }
+
+    // retire the whole packet: the epilogue runs with all 32 lanes
+    uint32_t payload[PW > 0 ? PW : 1];
+    float max_t = 0.0f;
+    if (valid) {
+      max_t = __uint_as_float(lstk[DEPTH].x);
+#pragma unroll
+      for (int w = 0; w + 1 < PW; w += 2) {
+        const uint2 e = lstk[DEPTH + 1 + w / 2];
+        payload[w] = e.x;
+        payload[w + 1] = e.y;
+      }
+      if (PW & 1) payload[PW - 1] = lstk[DEPTH + 1 + PW / 2].x;
+    }
+    epi(valid, (size_t)mine, best.t, best.u, best.v, best.prim, max_t, payload);
+  }
+}
+
 }  // namespace nrt

@@ -16,7 +16,7 @@ for l in sass.splitlines():
     m = re.match(r"\s*/\*[0-9a-f]+\*/\s+(@!?U?P\d\s+)?([A-Z0-9_.]+)", l)
     if cur and m:
         ops[cur].append(m.group(2))
-WANT = ["traverse_fast3_kernel", "traverse_conformance_kernelINS_7AosRaysELb0", "scene_unified_kernelILi64ELi8E", "scene_list_kernel", "traverse_f64_kernel", "bin_large_kernel", "subtree_kernel",
+WANT = ["traverse_fast3_kernel", "traverse_packet_kernel", "traverse_conformance_kernelINS_7AosRaysELb0", "scene_unified_kernelILi64ELi8E", "scene_list_kernel", "traverse_f64_kernel", "bin_large_kernel", "subtree_kernel",
         "instance_setup_kernel"]
 print("| kernel | SASS instrs | FFMA/DFMA | ... of them within a division / sqrt sequence | FMUL+FADD (DMUL+DADD) | MUFU | REDUX | MATCH |")
 print("|---|---|---|---|---|---|---|---|")
