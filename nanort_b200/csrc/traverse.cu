@@ -147,10 +147,11 @@ typedef Policy3<10, 24, true, 8, false, 2> DefaultPolicy;
 // the precomputed face normals: MINB 9/10 x NODE_UNROLL 2/3 all lie within 1 % of each other on the bench headline
 // (10 spills 32 B at 48 registers), so this row stays (DESIGN.md section 10).
 typedef Policy3<9, 32, true, 12, true, 3> CameraPolicy;
-// The packet walk of the camera launch over the camera-relative copies (traverse_packet_kernel): 9 CTAs per SM, 56
-// registers and no spills; 10 (48 registers) spills 16 B and lies within 1 %, 12 (40 registers) is 2 % slower
-// (DESIGN.md section 10).
-typedef PacketPolicy<9> CameraPacketPolicy;
+// The packet walk of the camera launch over the camera-relative copies (traverse_packet_kernel): two samples per lane,
+// 7 CTAs per SM (72 registers, 28 B spilled).  Swept on H100 (80GB HBM3, 700 W; DESIGN.md section 10): one sample per
+// lane at 9 CTAs (56 registers) is 5 % slower on the bench headline; two samples at 6 CTAs (80 registers, no spills)
+// 2 %; at 8 and 9 CTAs they spill 92 B and more.
+typedef PacketPolicy<7, 2> CameraPacketPolicy;
 typedef Policy3<10, 20, false, 12, false, 3> IncoherentPolicy;
 typedef Policy3<9, 32, false, 12, true, 3> IncoherentCameraPolicy;
 // The path tracer's radiance launch: its retire step IS the shading block, which needs more registers than the plain
@@ -308,12 +309,16 @@ static int launch_fused(const Accel *a, Rays rays, size_t n, const unsigned long
 template <int DEPTH>
 static cudaError_t launch_packet(const Accel *a, CameraRays rays, size_t n, const PrimaryToAoEpilogue &epi,
                                  const TraceOptions16 &opt, uint32_t flags, unsigned long long *cursor, cudaStream_t s) {
+  typedef CameraUnits<CameraPacketPolicy::kRays> Units;
+  const Units units(epi.p);
+  const size_t n_units = units.count(n);  // one warp each
   const size_t warps_per_block = kTraverseBlock / 32;
   size_t grid = (size_t)device_sm_count(a->device) * CameraPacketPolicy::kMinBlocks;
-  const size_t need_blocks = ((n + 31) / 32 + warps_per_block - 1) / warps_per_block;
+  const size_t need_blocks = (n_units + warps_per_block - 1) / warps_per_block;
   if (grid > need_blocks) grid = need_blocks;
-  traverse_packet_kernel<CameraRays, DEPTH, CameraPacketPolicy, PrimaryToAoEpilogue>
-      <<<(unsigned)grid, kTraverseBlock, 0, s>>>(a->d_pair_rel, a->d_tris_rel, rays, n, epi, opt, flags, cursor);
+  traverse_packet_kernel<CameraRays, Units, DEPTH, CameraPacketPolicy, PrimaryToAoEpilogue>
+      <<<(unsigned)grid, kTraverseBlock, 0, s>>>(a->d_pair_rel, a->d_tris_rel, rays, units, n_units, n, epi, opt, flags,
+                                                 cursor);
   return cudaGetLastError();
 }
 

@@ -208,6 +208,33 @@ struct CameraRaysT {
 typedef CameraRaysT<true> CameraRays;      // over the camera-relative copies
 typedef CameraRaysT<false> CameraRaysAbs;  // over the accel's own arrays
 
+// Work units of the packet walk (traverse_packet_kernel): one 8x4 block of one tile at K consecutive samples.  Unit u
+// of a wave is tile u / per_tile, sample group j and block blk (u % per_tile = j * blocks + blk), and its ray (r, lane)
+// is slot  tile * tile_slots + (K * j + r) * tile_pix + blk * 32 + lane  of CameraRaysT's order.  A sample K * j + r
+// past spp is no ray (spp not a multiple of K).
+template <int K>
+struct CameraUnits {
+  FastDiv per_tile, blocks;  // units per tile (ceil(spp / K) sample groups of every block), 8x4 blocks per tile
+  uint32_t tile_pix, tile_slots, spp;
+  __host__ explicit CameraUnits(const nrt_ao_params &p) {
+    tile_pix = p.tile_w * p.tile_h;
+    tile_slots = tile_pix * p.spp;
+    spp = p.spp;
+    blocks = FastDiv(tile_pix / 32);
+    per_tile = FastDiv((p.spp + K - 1) / K * (tile_pix / 32));
+  }
+  // units of a wave of n_slots slots (whole tiles)
+  __host__ size_t count(size_t n_slots) const { return (n_slots + tile_slots - 1) / tile_slots * per_tile.d; }
+  __device__ __forceinline__ bool slot(uint32_t unit, int r, uint32_t lane, uint32_t &s) const {
+    uint32_t k, rem, j, blk;
+    per_tile.divmod(unit, k, rem);
+    blocks.divmod(rem, j, blk);
+    const uint32_t smp = (uint32_t)K * j + (uint32_t)r;
+    s = k * tile_slots + smp * tile_pix + blk * 32u + lane;
+    return smp < spp;
+  }
+};
+
 // Unit normalize(cross(v1 - v0, v2 - v0)) of a triangle (zero for a degenerate one) and twice its area.
 __device__ __forceinline__ void geometric_normal(const float *__restrict__ verts, const uint32_t *__restrict__ faces,
                                                  uint32_t prim, float &nx, float &ny, float &nz, float &area2) {
