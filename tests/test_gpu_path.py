@@ -12,6 +12,8 @@ glibc differ in the last bit).  The bounce's continuation rays -- the DEVICE's -
 import numpy as np
 import pytest
 
+import ao_model as M
+
 pytestmark = pytest.mark.gpu
 
 TILE = (64, 8)
@@ -21,7 +23,8 @@ def _rel(a, b, floor=1e-3):
     return float(np.max(np.abs(a - b) / np.maximum(np.abs(b), floor))) if a.size else 0.0
 
 
-def _setup(torch, api, S, v, f, mats, ids, emissive, fvn, W, H, spp, bounces, seed, camera="cornell", build_flags=0):
+def _setup(torch, api, S, v, f, mats, ids, emissive, fvn, W, H, spp, bounces, seed, camera="cornell", build_flags=0,
+           tile=TILE, sample0=0, shard=0, n_shards=1):
     acc = api.BVHAccel()
     acc.Build(len(f), v, f, flags=build_flags)
     keep = {"m": torch.as_tensor(np.ascontiguousarray(mats).view(np.float32).reshape(-1), device="cuda"),
@@ -32,8 +35,8 @@ def _setup(torch, api, S, v, f, mats, ids, emissive, fvn, W, H, spp, bounces, se
     cam = S.scene_camera(camera, W, H)
     for i in range(12):
         p.cam[i] = float(cam[i])
-    p.width, p.height, p.spp, p.sample0, p.seed = W, H, spp, 0, seed
-    p.tile_w, p.tile_h, p.shard, p.n_shards = TILE[0], TILE[1], 0, 1
+    p.width, p.height, p.spp, p.sample0, p.seed = W, H, spp, sample0, seed
+    p.tile_w, p.tile_h, p.shard, p.n_shards = tile[0], tile[1], shard, n_shards
     p.max_bounces, p.ray_min_t, p.ray_max_t = bounces, 1e-3, 1e30
     p.n_materials, p.n_emissive = len(mats), len(emissive)
     p.d_materials, p.d_material_ids, p.d_emissive_faces = keep["m"].data_ptr(), keep["i"].data_ptr(), keep["e"].data_ptr()
@@ -41,14 +44,23 @@ def _setup(torch, api, S, v, f, mats, ids, emissive, fvn, W, H, spp, bounces, se
     return acc, p, cam, keep
 
 
-def _bounce_by_bounce(with_normals, scene="cornell", build_flags=0, min_depth=0):
+def _bounce_by_bounce(with_normals, scene="cornell", build_flags=0, min_depth=0, frame=None, slots=None):
+    """scene: "cornell", "terrain" or a (verts, faces, materials, material_ids, emissive_faces) tuple seen by the Cornell
+    camera.  frame: overrides of the tile map {W, H, spp, bounces, seed, tile, sample0, shard, n_shards} and of the
+    camera block (cam).  slots: the shard's global slots whose paths are traced (default: every slot inside the
+    image); path id = global slot."""
     import torch
     from oracle import orc
-    from nanort_b200 import api, dist as nd, scenes as S
+    from nanort_b200 import api, scenes as S
 
     if not orc.ReferencePathTracer.available():
         pytest.skip("oracle/_ref/libpt_ref.so not built (no reference tree at build time)")
-    if scene == "cornell":
+    terrain = isinstance(scene, str) and scene == "terrain"
+    camera = "terrain" if terrain else "cornell"
+    if not isinstance(scene, str):
+        v, f, mats, ids, emissive = scene
+        W, H, spp, bounces, seed = 64, 48, 4, 8, 5
+    elif scene == "cornell":
         v, f, mats, ids, emissive = S.cornell_with_materials()
         W, H, spp, bounces, seed = 64, 48, 4, 8, 5
     else:  # BASELINE.json configs[2]: the 1,002,528-triangle terrain under an area light, as bench.py sets it up
@@ -59,23 +71,30 @@ def _bounce_by_bounce(with_normals, scene="cornell", build_flags=0, min_depth=0)
         ids[l0:] = 1
         emissive = np.arange(l0, l0 + ln, dtype=np.uint32)
         W, H, spp, bounces, seed = 192, 108, 2, 6, 3
+    cfg = dict(W=W, H=H, spp=spp, bounces=bounces, seed=seed, tile=TILE, sample0=0, shard=0, n_shards=1, cam=None)
+    cfg.update(frame or {})
+    W, H, spp, bounces, seed, tile = (cfg[k] for k in ("W", "H", "spp", "bounces", "seed", "tile"))
     ref = orc.ReferencePathTracer(v, f, ids, mats)  # face normals as the example's loader makes them (calcNormal)
     assert np.array_equal(ref.emissive_faces(), emissive), "MeshLight's emissive-face list != the list handed to the device"
     fvn = ref.fvn if with_normals else None
-    acc, p, cam, keep = _setup(torch, api, S, v, f, mats, ids, emissive, fvn, W, H, spp, bounces, seed, camera=scene,
-                               build_flags=build_flags)
+    acc, p, cam, keep = _setup(torch, api, S, v, f, mats, ids, emissive, fvn, W, H, spp, bounces, seed, camera=camera,
+                               build_flags=build_flags, tile=tile, sample0=cfg["sample0"], shard=cfg["shard"],
+                               n_shards=cfg["n_shards"])
     assert acc.GetStatistics()["max_tree_depth"] >= min_depth
+    if cfg["cam"] is not None:
+        cam = np.asarray(cfg["cam"], np.float32)
+        for i in range(12):
+            p.cam[i] = float(cam[i])
 
-    # bounce 0 input: the camera rays of every slot (slot = path id), weight 1, do_emission = true
-    pix_of_slot, smp_of_slot = nd.slot_pixels(W, H, TILE[0], TILE[1], 0, 1, spp)
+    # bounce 0 input: the camera rays of the slots (slot = path id), weight 1, do_emission = true
+    pix_of_slot, smp_of_slot = M.slots(W, H, tile[0], tile[1], spp, cfg["sample0"], cfg["shard"], cfg["n_shards"])
     n_slots = len(pix_of_slot)
-    valid = np.nonzero(pix_of_slot >= 0)[0]
-    order = np.argsort(pix_of_slot[valid] * spp + smp_of_slot[valid], kind="stable")
-    rays0 = S.primary_rays(cam, W, H, spp=spp, seed=seed)  # ray index = pixel * spp + sample
+    valid = np.nonzero(pix_of_slot >= 0)[0] if slots is None else np.asarray(slots, np.int64)
+    assert len(valid) and np.all(pix_of_slot[valid] >= 0), "only slots inside the image carry a camera ray"
+    order = np.lexsort((smp_of_slot[valid], pix_of_slot[valid]))  # ray order: pixel, then sample
     pid = valid[order].astype(np.uint32)
-    assert len(rays0) == len(pid)
-    org = rays0["org"].astype(np.float32)
-    dirs = rays0["dir"].astype(np.float32)
+    org = np.broadcast_to(np.asarray(cam[:3], np.float32), (len(pid), 3)).copy()
+    dirs = M.camera_dirs(cam, W, H, seed, pix_of_slot[pid], smp_of_slot[pid]).astype(np.float32)
     dev = "cuda"
 
     def f4(xyz, w):
@@ -98,7 +117,7 @@ def _bounce_by_bounce(with_normals, scene="cornell", build_flags=0, min_depth=0)
         sh_o = torch.zeros((n, 4), dtype=torch.float32, device=dev)
         sh_d = torch.zeros((n, 4), dtype=torch.float32, device=dev)
         sh_c = torch.zeros((n, 4), dtype=torch.float32, device=dev)
-        w_in = d_weight.cpu().numpy()[pid]
+        w_in = d_weight[torch.as_tensor(pid.astype(np.int64), device=dev)].cpu().numpy()
         accum_before = accum.cpu().numpy().reshape(-1, 3).astype(np.float64)
         n_cont, n_sh = acc.PathBounce(p, b, n, d_o.data_ptr(), d_d.data_ptr(), d_pid.data_ptr(), d_weight.data_ptr(),
                                       out_o.data_ptr(), out_d.data_ptr(), out_pid.data_ptr(), sh_o.data_ptr(),
@@ -128,9 +147,9 @@ def _bounce_by_bounce(with_normals, scene="cornell", build_flags=0, min_depth=0)
         gsort, rsort = np.argsort(got_pid), np.argsort(ref_pid)
         assert _rel(go[gsort][:, :3], want["next_org"][cont][rsort]) <= 1e-5
         assert float(np.max(np.abs(gd[gsort][:, :3] - want["next_dir"][cont][rsort]))) <= 2e-5 if n_cont else True
-        w_out = d_weight.cpu().numpy()
-        assert _rel(w_out[ref_pid][:, :3], want["weight"][cont][:, :3], floor=1e-6) <= 1e-5
-        assert np.array_equal(w_out[ref_pid][:, 3] != 0, want["weight"][cont][:, 3] != 0), "do_emission flag"
+        w_out = d_weight[torch.as_tensor(ref_pid.astype(np.int64), device=dev)].cpu().numpy()
+        assert _rel(w_out[:, :3], want["weight"][cont][:, :3], floor=1e-6) <= 1e-5
+        assert np.array_equal(w_out[:, 3] != 0, want["weight"][cont][:, 3] != 0), "do_emission flag"
         # ---- shadow rays: matched by (pixel, origin): sort both by the contribution's pixel and the ray origin bits
         gs_o, gs_d, gs_c = sh_o.cpu().numpy()[:n_sh], sh_d.cpu().numpy()[:n_sh], sh_c.cpu().numpy()[:n_sh]
         got_pix = gs_c[:, 3].copy().view(np.uint32)
@@ -161,8 +180,8 @@ def _bounce_by_bounce(with_normals, scene="cornell", build_flags=0, min_depth=0)
         # next bounce: the DEVICE's continuation queue
         pid = got_pid
         org, dirs = go[:, :3].copy(), gd[:, :3].copy()
-    assert total_checked > (15000 if scene == "cornell" else 25000) and ("shadow", True) in lobes_seen
-    assert scene != "cornell" or ("emit", True) in lobes_seen  # the terrain's light is outside the camera's view
+    assert total_checked > (25000 if terrain else 15000) and ("shadow", True) in lobes_seen
+    assert terrain or ("emit", True) in lobes_seen  # the terrain's light is outside the camera's view
     return total_checked
 
 
