@@ -61,6 +61,9 @@ EXPORTS = [
     "nrt_probe_read_gbs", "nrt_probe_copy_gbs", "nrt_traverse_lane_stats_device", "nrt_build_f64_ex",
 ]
 
+# every symbol include/nanort_b200_scene_path.h declares (the path tracer over two-level scenes)
+SCENE_PATH_EXPORTS = ["nrt_scene_render_path_device", "nrt_scene_path_bounce_device"]
+
 
 class NanortB200Error(RuntimeError):
     pass
@@ -101,6 +104,12 @@ class PathParams(C.Structure):
         ("d_facevarying_normals", C.c_void_p),
         ("flags", C.c_uint32), ("pad", C.c_uint32),
     ]
+
+
+class SceneShading(C.Structure):
+    """nrt_scene_shading: one instance's material ids (uint32 per face) and face-varying normals (float[9] per face,
+    instance-local), device pointers or None."""
+    _fields_ = [("d_material_ids", C.c_void_p), ("d_facevarying_normals", C.c_void_p)]
 
 
 class PathResult(C.Structure):
@@ -157,6 +166,9 @@ def lib():
     L.nrt_scene_traverse.argtypes = [vp, vp, sz, vp, vp, u32]
     L.nrt_scene_traverse_device.argtypes = [vp, vp, sz, vp, vp, u32, vp]
     L.nrt_scene_render_ao_device.argtypes = [vp, vp, vp, vp, vp]
+    L.nrt_scene_render_path_device.argtypes = [vp, C.POINTER(PathParams), vp, vp, C.POINTER(PathResult), vp]
+    L.nrt_scene_path_bounce_device.argtypes = [vp, C.POINTER(PathParams), vp, u32, C.c_uint64] + [vp] * 11 + [u64p, u64p,
+                                                                                                    C.c_int, vp]
     L.nrt_build_f64.argtypes = [vp, sz, sz, vp, u32, vp, C.POINTER(vp)]
     L.nrt_build_f64_ex.argtypes = [vp, sz, sz, vp, u32, vp, u32, C.POINTER(vp)]
     L.nrt_adopt_f64.argtypes = [vp, sz, vp, sz, vp, sz, sz, vp, u32, C.POINTER(vp)]
@@ -613,6 +625,36 @@ class Scene:
         _check(lib().nrt_scene_render_ao_device(self._h, C.byref(params), C.c_void_p(d_accum_ptr), C.byref(res),
                                                 C.c_void_p(stream) if stream else None))
         return res
+
+    def _shading(self, shading):
+        assert len(shading) == len(self._nodes), "one SceneShading per instance"
+        arr = (SceneShading * len(shading))()
+        for i, sh in enumerate(shading):
+            arr[i] = sh
+        return arr
+
+    def RenderPath(self, params: "PathParams", shading, d_accum_rgb_ptr, stream=None):
+        """Path tracing over the two-level scene (nrt_scene_render_path_device): BVHAccel.RenderPath's parameters with
+        params.d_emissive_faces = {instance, face} pairs and per-instance `shading` (a list of SceneShading)."""
+        res = PathResult()
+        _check(lib().nrt_scene_render_path_device(self._h, C.byref(params), C.cast(self._shading(shading), C.c_void_p),
+                                                  C.c_void_p(d_accum_rgb_ptr), C.byref(res),
+                                                  C.c_void_p(stream) if stream else None))
+        return res
+
+    def PathBounce(self, params: "PathParams", shading, bounce, n_rays, d_org_tmin, d_dir_tmax, d_path_id, d_weight,
+                   d_out_org_tmin, d_out_dir_tmax, d_out_path_id, d_sh_org_tmin, d_sh_dir_tmax, d_sh_contrib_pix,
+                   d_accum_rgb, skip_shadow_pass=False, stream=None):
+        """nrt_scene_path_bounce_device: one bounce on caller-owned device queues; returns (n_continue, n_shadow)."""
+        nc, ns = C.c_uint64(0), C.c_uint64(0)
+        vp = C.c_void_p
+        _check(lib().nrt_scene_path_bounce_device(self._h, C.byref(params), C.cast(self._shading(shading), vp), int(bounce),
+                                                  int(n_rays), vp(d_org_tmin), vp(d_dir_tmax), vp(d_path_id), vp(d_weight),
+                                                  vp(d_out_org_tmin), vp(d_out_dir_tmax), vp(d_out_path_id),
+                                                  vp(d_sh_org_tmin), vp(d_sh_dir_tmax), vp(d_sh_contrib_pix),
+                                                  vp(d_accum_rgb), C.byref(nc), C.byref(ns), 1 if skip_shadow_pass else 0,
+                                                  vp(stream) if stream else None))
+        return int(nc.value), int(ns.value)
 
 
 # ------------------------------------------------------------------ BVHAccel<double>

@@ -72,6 +72,13 @@ __global__ void end_bounce_kernel(const unsigned long long *counters, unsigned l
 }
 
 }  // namespace
+
+// the camera stage on its own, for the two-level scene's path pass (scene.cu)
+void launch_path_camera(const nrt_path_params &p, unsigned long long slot0, uint32_t count, const PathQueues &q,
+                        unsigned long long *counters, cudaStream_t s) {
+  gen_camera_kernel<<<(count + 255) / 256, 256, 0, s>>>(p, slot0, count, q, counters);
+}
+
 }  // namespace nrt
 
 using namespace nrt;

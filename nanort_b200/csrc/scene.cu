@@ -27,7 +27,9 @@
 #include <algorithm>
 #include <cstring>
 #include <new>
+#include <vector>
 
+#include "../../include/nanort_b200_scene_path.h"
 #include "common.cuh"
 #include "trav_common.cuh"
 #include "nodehits.cuh"
@@ -602,6 +604,7 @@ struct Scene {
   InstanceDev *d_inst = nullptr;
   float *d_state = nullptr;  // 76 floats per instance
   uint32_t max_blas_depth = 0;
+  std::vector<uint32_t> n_faces;  // per instance: triangles of its accel
   // per-launch scratch of the ring's slot k: the ray cursor d_counters[k], the overflow count d_counters[4 + k] and its
   // own overflow list
   static constexpr int kSlots = 4;
@@ -756,6 +759,7 @@ int nrt_scene_commit(const nrt_instance *instances, uint32_t n_instances, uint32
       h[i].verts = a->d_verts;
       h[i].faces = a->d_faces;
       sc->max_blas_depth = std::max(sc->max_blas_depth, a->stats.max_tree_depth);
+      sc->n_faces.push_back(a->d_faces ? (uint32_t)a->n_prims : 0u);  // 0: not a triangle accel
     }
     e = cudaMemcpyAsync(d_in, h.data(), sizeof(InstanceIn) * (size_t)n_instances, cudaMemcpyHostToDevice, sc->stream);
     if (e == cudaSuccess) {
@@ -1087,5 +1091,465 @@ extern "C" int nrt_scene_render_ao_device(const nrt_scene *s, const nrt_ao_param
     res->launches = launches;
     res->traverse_launches = trav_launches;
   }
+  return NRT_OK;
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Path tracing over a two-level scene (nrt_scene_render_path_device, nrt_scene_path_bounce_device): path.cu's wavefront
+// loop with nrt_scene_traverse_device as its traversal step, as stand-alone stage kernels.  The shading of a hit is
+// path_shade_hit (wavefront.cuh), the block the flat pass runs in its retire step, fed with world-space geometry:
+// P = org + t dir from the world ray and world distance, the hit triangle moved to world space by the instance's
+// matrix, its face-varying normals by the instance's inverse_transpose33, the lights from world-space records.
+// Spawned rays are lifted off the surface like the AO pass's (nanosg walks an instance with the local range
+// {0, FLT_MAX}, so min_t cannot keep a ray off the surface it starts on).
+namespace nrt {
+
+void launch_path_camera(const nrt_path_params &p, unsigned long long slot0, uint32_t count, const PathQueues &q,
+                        unsigned long long *counters, cudaStream_t s);
+
+namespace {
+
+struct SceneShadingDev {  // nrt_scene_shading
+  const uint32_t *mat_ids;
+  const float *fvn;
+};
+static_assert(sizeof(SceneShadingDev) == sizeof(nrt_scene_shading), "nrt_scene_shading");
+
+// One emissive pair in world space, 64 bytes: v0.xyz v1.x | v1.yz v2.xy | v2.z n.xyz | area e.xyz (n: unit
+// cross(e1, e2), area: half its length before normalisation -- geometric_normal() of the world triangle)
+struct SceneLights {
+  const float4 *rec;
+  __device__ __forceinline__ void sample(uint32_t k, float c0, float c1, float c2, float Px, float Py, float Pz,
+                                         float &lx, float &ly, float &lz, float &lnx, float &lny, float &lnz,
+                                         float &area, float &ex, float &ey, float &ez) const {
+    const float4 a = __ldg(rec + 4 * (size_t)k), b = __ldg(rec + 4 * (size_t)k + 1), c = __ldg(rec + 4 * (size_t)k + 2),
+                 d = __ldg(rec + 4 * (size_t)k + 3);
+    lx = c0 * a.x + c1 * a.w + c2 * b.z - Px;
+    ly = c0 * a.y + c1 * b.x + c2 * b.w - Py;
+    lz = c0 * a.z + c1 * b.y + c2 * c.x - Pz;
+    lnx = c.y;
+    lny = c.z;
+    lnz = c.w;
+    area = d.x;
+    ex = d.y;
+    ey = d.z;
+    ez = d.w;
+  }
+};
+
+// Spawned rays start lift = ray_min_t above P along the unit geometric normal g, on the side the ray leaves.
+struct SceneSpawn {
+  float gx, gy, gz;
+  __device__ __forceinline__ void lifted(float lift, float Px, float Py, float Pz, float dx, float dy, float dz,
+                                          float &x, float &y, float &z) const {
+    float nx = gx, ny = gy, nz = gz;
+    const float c = nx * dx + ny * dy + nz * dz;
+    if (c < 0.0f) nx = -nx, ny = -ny, nz = -nz;
+    x = Px + nx * lift;
+    y = Py + ny * lift;
+    z = Pz + nz * lift;
+  }
+  __device__ __forceinline__ void continuation(const nrt_path_params &p, float Px, float Py, float Pz, float ox,
+                                               float oy, float oz, float4 &co, float4 &cd) const {
+    float x, y, z;
+    lifted(p.ray_min_t, Px, Py, Pz, ox, oy, oz, x, y, z);
+    co = make_float4(x, y, z, p.ray_min_t);
+    cd = make_float4(ox, oy, oz, p.ray_max_t);
+    if (ox == 0.0f && oy == 0.0f && oz == 0.0f) {  // total internal reflection: a radiance ray that misses at the root
+      co.w = 0.0f;
+      cd.w = -1.0f;
+    }
+  }
+  // Direction and dist come from the unlifted P.  The lifted ray meets the light triangle's plane (unit normal ln) at
+  // dist - ray_min_t (ln . g') / (ln . l) rather than at dist (g' = the lift's direction), so that is where max_t is put,
+  // less 1e-5: with dist - 1e-5 the light would occlude its own sample.  A light seen edge-on (ln . l = 0) adds nothing.
+  __device__ __forceinline__ void shadow(const nrt_path_params &p, float Px, float Py, float Pz, float lx, float ly,
+                                         float lz, float dist, float lnx, float lny, float lnz, float4 &so,
+                                         float4 &sd) const {
+    float x, y, z;
+    lifted(p.ray_min_t, Px, Py, Pz, lx, ly, lz, x, y, z);
+    const float ndl = lnx * lx + lny * ly + lnz * lz;
+    const float ndo = lnx * (x - Px) + lny * (y - Py) + lnz * (z - Pz);  // ray_min_t (ln . g')
+    so = make_float4(x, y, z, 0.00001f);
+    sd = make_float4(lx, ly, lz, (ndl != 0.0f ? dist - ndo / ndl : dist) - 0.00001f);
+  }
+};
+
+// t[k] = ((m[0][k] v0 + m[1][k] v1) + m[2][k] v2) + m[3][k] over a full row-major 4x4 (Matrix::MultV)
+__device__ __forceinline__ void multv16(const float *m, float x, float y, float z, float &ox, float &oy, float &oz) {
+  ox = ((m[0] * x + m[4] * y) + m[8] * z) + m[12];
+  oy = ((m[1] * x + m[5] * y) + m[9] * z) + m[13];
+  oz = ((m[2] * x + m[6] * y) + m[10] * z) + m[14];
+}
+
+__device__ __forceinline__ void world_triangle(const InstanceDev *I, uint32_t prim, float w[9]) {
+  const Mat43 xf = load_mat(&I->xf);
+  const uint32_t *f = I->faces + 3 * (size_t)prim;
+  for (int k = 0; k < 3; k++) {
+    const float *v = I->verts + 3 * (size_t)f[k];
+    multv(xf, v[0], v[1], v[2], w[3 * k], w[3 * k + 1], w[3 * k + 2]);
+  }
+}
+
+// unit cross(e1, e2) of a world triangle and the length of the cross product (geometric_normal's arithmetic)
+__device__ __forceinline__ void world_normal(const float w[9], float &nx, float &ny, float &nz, float &area2) {
+  const float e1x = w[3] - w[0], e1y = w[4] - w[1], e1z = w[5] - w[2];
+  const float e2x = w[6] - w[0], e2y = w[7] - w[1], e2z = w[8] - w[2];
+  nx = e1y * e2z - e1z * e2y;
+  ny = e1z * e2x - e1x * e2z;
+  nz = e1x * e2y - e1y * e2x;
+  area2 = sqrtf(nx * nx + ny * ny + nz * nz);
+  const float il = area2 > 0.0f ? 1.0f / area2 : 0.0f;
+  nx *= il;
+  ny *= il;
+  nz *= il;
+}
+
+__global__ void __launch_bounds__(128)
+    scene_light_setup_kernel(const uint32_t *__restrict__ pairs, uint32_t n, const InstanceDev *__restrict__ inst,
+                             const SceneShadingDev *__restrict__ shading, const PathMaterial *__restrict__ mats,
+                             float4 *__restrict__ rec) {
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const uint32_t node = pairs[2 * (size_t)k], prim = pairs[2 * (size_t)k + 1];
+  float w[9], nx, ny, nz, a2;
+  world_triangle(inst + node, prim, w);
+  world_normal(w, nx, ny, nz, a2);
+  const uint32_t *ids = shading[node].mat_ids;
+  const PathMaterial &m = mats[ids ? ids[prim] : 0u];
+  rec[4 * (size_t)k + 0] = make_float4(w[0], w[1], w[2], w[3]);
+  rec[4 * (size_t)k + 1] = make_float4(w[4], w[5], w[6], w[7]);
+  rec[4 * (size_t)k + 2] = make_float4(w[8], nx, ny, nz);
+  rec[4 * (size_t)k + 3] = make_float4(0.5f * a2, m.emission[0], m.emission[1], m.emission[2]);
+}
+
+__global__ void __launch_bounds__(256)
+    scene_pack_rays_kernel(const float4 *__restrict__ org_tmin, const float4 *__restrict__ dir_tmax, uint32_t n,
+                           Ray36 *__restrict__ rays) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float4 o = org_tmin[i], d = dir_tmax[i];
+  Ray36 r;
+  r.org[0] = o.x, r.org[1] = o.y, r.org[2] = o.z;
+  r.dir[0] = d.x, r.dir[1] = d.y, r.dir[2] = d.z;
+  r.min_t = o.w, r.max_t = d.w;
+  r.type = 0;
+  rays[i] = r;
+}
+
+// the shading of the n radiance rays of queue `in` from their scene hit records
+__global__ void __launch_bounds__(256)
+    scene_path_shade_kernel(nrt_path_params p, unsigned long long slot0, uint32_t bounce, uint32_t n, PathQueues q,
+                            int in, const SceneHit32 *__restrict__ hits, const uint8_t *__restrict__ mask,
+                            const InstanceDev *__restrict__ inst, const float *__restrict__ state76,
+                            const SceneShadingDev *__restrict__ shading, const float4 *__restrict__ lights,
+                            float *accum, unsigned long long *counters) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  bool cont = false, shadow = false;
+  float4 co = make_float4(0, 0, 0, 0), cd = co, so = co, sd = co, sc = co;
+  uint32_t pid = 0, pix, smp;
+  if (i < n && mask[i]) {
+    pid = q.path_id[in][i];
+    if (slot_to_pixel(tile_map(p), slot0 + pid, pix, smp)) {
+      smp += p.sample0;
+      const float4 o = q.org_tmin[in][i], d = q.dir_tmax[in][i];
+      const SceneHit32 h = hits[i];
+      const SceneShadingDev sh = shading[h.node_id];
+      float w[9], gx, gy, gz, a2;
+      world_triangle(inst + h.node_id, h.prim_id, w);
+      world_normal(w, gx, gy, gz, a2);
+      float nx, ny, nz;
+      if (sh.fvn) {  // vertex normals to world space (nanosg.h:866-867), then main.cc:862-875
+        const float *T = state76 + 76 * (size_t)h.node_id + 48;  // inverse_transpose33
+        const float *n0 = sh.fvn + 9 * (size_t)h.prim_id;
+        float wn[9];
+        for (int k = 0; k < 3; k++) multv16(T, n0[3 * k], n0[3 * k + 1], n0[3 * k + 2], wn[3 * k], wn[3 * k + 1], wn[3 * k + 2]);
+        const float b0 = 1.0f - h.u - h.v;
+        nx = b0 * wn[0] + h.u * wn[3] + h.v * wn[6];
+        ny = b0 * wn[1] + h.u * wn[4] + h.v * wn[7];
+        nz = b0 * wn[2] + h.u * wn[5] + h.v * wn[8];
+        const float l = sqrtf(nx * nx + ny * ny + nz * nz);
+        if (fabsf(l) > 1.0e-6f) {
+          const float il = 1.0f / l;
+          nx *= il;
+          ny *= il;
+          nz *= il;
+        }
+      } else {  // calcNormal's orientation, -cross(e1, e2), as the flat pass
+        nx = -gx;
+        ny = -gy;
+        nz = -gz;
+      }
+      const PathMaterial *mats = reinterpret_cast<const PathMaterial *>(p.d_materials);
+      path_shade_hit(p, bounce, pix, smp, o, d, h.t, nx, ny, nz, mats + (sh.mat_ids ? sh.mat_ids[h.prim_id] : 0u),
+                     SceneLights{lights}, SceneSpawn{gx, gy, gz}, q.weight[pid], q.weight + pid, accum, cont, shadow, co,
+                     cd, so, sd, sc);
+    }
+  }
+  path_append(q, in ^ 1, counters, cont, shadow, pid, co, cd, so, sd, sc);
+}
+
+// shadow rays: occluded iff the scene walk reports a hit nearer than max_t (SceneSpawn::shadow)
+__global__ void __launch_bounds__(256)
+    scene_path_shadow_kernel(const SceneHit32 *__restrict__ hits, const uint8_t *__restrict__ mask,
+                             const float4 *__restrict__ sh_dir_tmax, const float4 *__restrict__ contrib_pix, uint32_t n,
+                             float *accum) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  if (mask[i] && hits[i].t < sh_dir_tmax[i].w) return;
+  const float4 c = contrib_pix[i];
+  const size_t pix = __float_as_uint(c.w);
+  atomicAdd(accum + 3 * pix + 0, c.x);
+  atomicAdd(accum + 3 * pix + 1, c.y);
+  atomicAdd(accum + 3 * pix + 2, c.z);
+}
+
+// What one call owns on the device: the per-instance shading table, the light records and the walk's buffers.
+struct ScenePathCall {
+  Scene *sc = nullptr;
+  nrt_path_params p{};
+  uint32_t trav_flags = 0;
+  SceneShadingDev *shading = nullptr;
+  float4 *lights = nullptr;
+  Ray36 *rays = nullptr;
+  SceneHit32 *hits = nullptr;
+  uint8_t *mask = nullptr;
+  unsigned long long *ctr = nullptr;  // [0] continuation rays, [1] shadow rays, [2] camera rays
+  uint32_t launches = 0, trav_launches = 0;
+  ~ScenePathCall() {
+    cudaFree(shading), cudaFree(lights), cudaFree(rays), cudaFree(hits), cudaFree(mask), cudaFree(ctr);
+  }
+};
+
+// Checks the arguments (nothing is launched when they are refused), reads the emissive pairs back, allocates the
+// call's buffers for `cap` rays and writes the shading table and the light records.
+int scene_path_begin(const char *name, const nrt_scene *s, const nrt_path_params *pp, const nrt_scene_shading *shading,
+                     size_t cap, cudaStream_t st, ScenePathCall &c) {
+  auto refuse = [&](const char *why) {
+    set_error(std::string(name) + ": " + why);
+    return NRT_ERR_INVALID;
+  };
+  if (!s || !pp) return refuse("NULL argument");
+  if (!shading) return refuse("NULL shading array (one nrt_scene_shading per instance)");
+  const nrt_path_params p = *pp;
+  if (p.width == 0 || p.height == 0 || p.spp == 0 || p.n_shards == 0 || p.shard >= p.n_shards || p.tile_w == 0 ||
+      p.tile_h == 0 || (p.tile_w % 8) != 0 || (p.tile_h % 4) != 0 || p.max_bounces == 0 || p.n_materials == 0 ||
+      !p.d_materials || (p.n_emissive > 0 && !p.d_emissive_faces))
+    return refuse("bad parameters");
+  if (p.d_material_ids || p.d_facevarying_normals)
+    return refuse("material ids and face-varying normals are given per instance (nrt_scene_shading), not in the params");
+  if (p.flags & NRT_TRAVERSE_ANY_HIT) return refuse("NRT_TRAVERSE_ANY_HIT is not supported by the scene walk");
+  if (p.flags & NRT_AO_PACKED_TILES) return refuse("NRT_AO_PACKED_TILES is not supported");
+  Scene *sc = const_cast<Scene *>(reinterpret_cast<const Scene *>(s));
+  for (uint32_t i = 0; i < sc->n; i++)
+    if (sc->n_faces[i] == 0) return refuse("triangle instances only");
+  c.sc = sc;
+  c.p = p;
+  c.trav_flags = p.flags & 0xFFFFu;
+  std::vector<uint32_t> pairs(2 * (size_t)p.n_emissive);
+  if (p.n_emissive) {
+    NRT_CUDA(cudaMemcpyAsync(pairs.data(), p.d_emissive_faces, sizeof(uint32_t) * pairs.size(), cudaMemcpyDeviceToHost,
+                             st));
+    NRT_CUDA(cudaStreamSynchronize(st));
+    for (uint32_t k = 0; k < p.n_emissive; k++)
+      if (pairs[2 * k] >= sc->n || pairs[2 * k + 1] >= sc->n_faces[pairs[2 * k]])
+        return refuse(("emissive pair " + std::to_string(k) + " is not an {instance, face} of the scene").c_str());
+  }
+  NRT_CUDA(cudaMalloc(&c.shading, sizeof(SceneShadingDev) * sc->n));
+  NRT_CUDA(cudaMalloc(&c.ctr, sizeof(unsigned long long) * 4));
+  NRT_CUDA(cudaMemcpyAsync(c.shading, shading, sizeof(SceneShadingDev) * sc->n, cudaMemcpyHostToDevice, st));
+  if (p.n_emissive && cap > 0) {
+    NRT_CUDA(cudaMalloc(&c.lights, 4 * sizeof(float4) * p.n_emissive));
+    scene_light_setup_kernel<<<(p.n_emissive + 127) / 128, 128, 0, st>>>(
+        static_cast<const uint32_t *>(p.d_emissive_faces), p.n_emissive, sc->d_inst, c.shading,
+        static_cast<const PathMaterial *>(p.d_materials), c.lights);
+    NRT_CUDA(cudaGetLastError());
+    c.launches++;
+  }
+  if (cap > 0) {
+    NRT_CUDA(cudaMalloc(&c.rays, sizeof(Ray36) * cap));
+    NRT_CUDA(cudaMalloc(&c.hits, sizeof(SceneHit32) * cap));
+    NRT_CUDA(cudaMalloc(&c.mask, cap));
+  }
+  return NRT_OK;
+}
+
+// One bounce: walk the n rays of queue `in`, shade them, read the counts; then walk the shadow rays and add the
+// visible light samples.  out[0] continuation rays, out[1] shadow rays, out[2] camera rays (ctr[2]).
+int scene_path_bounce(ScenePathCall &c, unsigned long long slot0, uint32_t bounce, uint32_t n, const PathQueues &q,
+                      int in, float *accum, bool shadow_pass, unsigned long long out[3], cudaStream_t st) {
+  const unsigned blocks = (n + 255) / 256;
+  NRT_CUDA(cudaMemsetAsync(c.ctr, 0, 2 * sizeof(unsigned long long), st));
+  scene_pack_rays_kernel<<<blocks, 256, 0, st>>>(q.org_tmin[in], q.dir_tmax[in], n, c.rays);
+  if (const int rc = scene_launch(c.sc, c.rays, n, c.hits, c.mask, c.trav_flags, st)) return rc;
+  scene_path_shade_kernel<<<blocks, 256, 0, st>>>(c.p, slot0, bounce, n, q, in, c.hits, c.mask, c.sc->d_inst,
+                                                  c.sc->d_state, c.shading, c.lights, accum, c.ctr);
+  NRT_CUDA(cudaGetLastError());
+  NRT_CUDA(cudaMemcpyAsync(out, c.ctr, 3 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  NRT_CUDA(cudaStreamSynchronize(st));  // the scene walk takes its ray count from the host
+  c.launches += 3;
+  c.trav_launches += 1;
+  const uint32_t ns = (uint32_t)out[1];
+  if (shadow_pass && ns > 0) {
+    const unsigned sb = (ns + 255) / 256;
+    scene_pack_rays_kernel<<<sb, 256, 0, st>>>(q.sh_org_tmin, q.sh_dir_tmax, ns, c.rays);
+    if (const int rc = scene_launch(c.sc, c.rays, ns, c.hits, c.mask, c.trav_flags, st)) return rc;
+    scene_path_shadow_kernel<<<sb, 256, 0, st>>>(c.hits, c.mask, q.sh_dir_tmax, q.sh_contrib_pix, ns, accum);
+    NRT_CUDA(cudaGetLastError());
+    c.launches += 3;
+    c.trav_launches += 1;
+  }
+  return NRT_OK;
+}
+
+}  // namespace
+}  // namespace nrt
+
+extern "C" int nrt_scene_render_path_device(const nrt_scene *s, const nrt_path_params *pp,
+                                            const nrt_scene_shading *shading, float *d_accum_rgb, nrt_path_result *res,
+                                            void *stream) {
+  if (!s || !pp || !d_accum_rgb) {
+    set_error("nrt_scene_render_path_device: NULL argument");
+    return NRT_ERR_INVALID;
+  }
+  const Scene *sc = reinterpret_cast<const Scene *>(s);
+  NRT_DEVICE(sc->device);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const nrt_path_params p = *pp;
+  // this shard's ray slots: whole tiles, dealt round-robin, in waves of whole tiles (nrt_scene_render_ao_device)
+  const unsigned long long tiles_x = p.tile_w ? (p.width + p.tile_w - 1) / p.tile_w : 0;
+  const unsigned long long tiles_y = p.tile_h ? (p.height + p.tile_h - 1) / p.tile_h : 0;
+  const unsigned long long n_tiles = tiles_x * tiles_y;
+  const unsigned long long my_tiles =
+      (p.n_shards && n_tiles > p.shard) ? (n_tiles - p.shard + p.n_shards - 1) / p.n_shards : 0;
+  const unsigned long long per_tile = (unsigned long long)p.tile_w * p.tile_h * p.spp;
+  const unsigned long long slots = my_tiles * per_tile;
+  unsigned long long wave =
+      per_tile ? std::max<unsigned long long>(per_tile, (((unsigned long long)1 << 22) / per_tile) * per_tile) : 0;
+  if (wave > slots) wave = slots;
+  if (wave > 0xFFFFFFF0ull) {
+    set_error("nrt_scene_render_path_device: a tile holds too many ray slots");
+    return NRT_ERR_INVALID;
+  }
+  ScenePathCall c;
+  int rc = scene_path_begin("nrt_scene_render_path_device", s, pp, shading, (size_t)wave, st, c);
+  if (rc != NRT_OK) {
+    cudaStreamSynchronize(st);  // nothing of a failed set-up may still use the buffers freed on return
+    return rc;
+  }
+  // per path: 2 radiance queues, the shadow queue, the throughput
+  PathQueues q;
+  std::vector<void *> bufs;
+  cudaError_t e = cudaSuccess;
+  auto alloc = [&](size_t bytes) -> void * {
+    void *ptr = nullptr;
+    if (e == cudaSuccess) e = cudaMalloc(&ptr, bytes ? bytes : 1);
+    bufs.push_back(ptr);
+    return ptr;
+  };
+  for (int k = 0; k < 2; k++) {
+    q.org_tmin[k] = static_cast<float4 *>(alloc(sizeof(float4) * wave));
+    q.dir_tmax[k] = static_cast<float4 *>(alloc(sizeof(float4) * wave));
+    q.path_id[k] = static_cast<uint32_t *>(alloc(sizeof(uint32_t) * wave));
+  }
+  q.sh_org_tmin = static_cast<float4 *>(alloc(sizeof(float4) * wave));
+  q.sh_dir_tmax = static_cast<float4 *>(alloc(sizeof(float4) * wave));
+  q.sh_contrib_pix = static_cast<float4 *>(alloc(sizeof(float4) * wave));
+  q.weight = static_cast<float4 *>(alloc(sizeof(float4) * wave));
+  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+  if (e == cudaSuccess) e = cudaEventCreate(&ev0);
+  if (e == cudaSuccess) e = cudaEventCreate(&ev1);
+  if (e == cudaSuccess) e = cudaEventRecord(ev0, st);
+  unsigned long long camera = 0, radiance = 0, shadow = 0;
+  for (unsigned long long slot0 = 0; slot0 < slots && e == cudaSuccess && rc == NRT_OK; slot0 += wave) {
+    const uint32_t count = (uint32_t)std::min(wave, slots - slot0);
+    e = cudaMemsetAsync(c.ctr, 0, 4 * sizeof(unsigned long long), st);
+    if (e != cudaSuccess) break;
+    launch_path_camera(p, slot0, count, q, c.ctr, st);
+    c.launches++;
+    uint32_t n = count;
+    int in = 0;
+    for (uint32_t b = 0; b < p.max_bounces && n > 0; b++) {
+      unsigned long long out[3];
+      rc = scene_path_bounce(c, slot0, b, n, q, in, d_accum_rgb, true, out, st);
+      if (rc != NRT_OK) break;
+      if (b == 0) camera += out[2];
+      radiance += b == 0 ? out[2] : n;  // slots outside the image are no Traverse calls
+      shadow += out[1];
+      n = (uint32_t)out[0];
+      in ^= 1;
+    }
+    if (e == cudaSuccess) e = cudaGetLastError();
+  }
+  float total_ms = 0.0f;
+  if (e == cudaSuccess && rc == NRT_OK) {
+    e = cudaEventRecord(ev1, st);
+    if (e == cudaSuccess) e = cudaEventSynchronize(ev1);
+    if (e == cudaSuccess) e = cudaEventElapsedTime(&total_ms, ev0, ev1);
+  } else {
+    cudaStreamSynchronize(st);  // nothing of a failed pass may still be running on the buffers freed below
+  }
+  if (ev0) cudaEventDestroy(ev0);
+  if (ev1) cudaEventDestroy(ev1);
+  for (void *ptr : bufs) cudaFree(ptr);
+  if (rc != NRT_OK) return rc;
+  NRT_CUDA(e);
+  if (res) {
+    res->camera_rays = camera;
+    res->radiance_rays = radiance;
+    res->shadow_rays = shadow;
+    res->traverse_ms = 0.0f;  // not split: the scene walk is timed as part of the pass
+    res->total_ms = total_ms;
+    res->launches = c.launches;
+    res->traverse_launches = c.trav_launches;
+  }
+  return NRT_OK;
+}
+
+extern "C" int nrt_scene_path_bounce_device(const nrt_scene *s, const nrt_path_params *pp,
+                                            const nrt_scene_shading *shading, uint32_t bounce, uint64_t n_rays,
+                                            const void *d_org_tmin, const void *d_dir_tmax, const uint32_t *d_path_id,
+                                            void *d_weight, void *d_out_org_tmin, void *d_out_dir_tmax,
+                                            uint32_t *d_out_path_id, void *d_sh_org_tmin, void *d_sh_dir_tmax,
+                                            void *d_sh_contrib_pix, float *d_accum_rgb, uint64_t *n_continue,
+                                            uint64_t *n_shadow, int skip_shadow_pass, void *stream) {
+  if (!s || !pp || !d_org_tmin || !d_dir_tmax || !d_path_id || !d_weight || !d_out_org_tmin || !d_out_dir_tmax ||
+      !d_out_path_id || !d_sh_org_tmin || !d_sh_dir_tmax || !d_sh_contrib_pix || !d_accum_rgb) {
+    set_error("nrt_scene_path_bounce_device: NULL argument");
+    return NRT_ERR_INVALID;
+  }
+  if (n_continue) *n_continue = 0;
+  if (n_shadow) *n_shadow = 0;
+  if (n_rays > 0xFFFFFFF0ull) {
+    set_error("nrt_scene_path_bounce_device: more than 2^32 - 16 rays");
+    return NRT_ERR_INVALID;
+  }
+  const Scene *sc = reinterpret_cast<const Scene *>(s);
+  NRT_DEVICE(sc->device);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  ScenePathCall c;
+  int rc = scene_path_begin("nrt_scene_path_bounce_device", s, pp, shading, (size_t)n_rays, st, c);
+  if (rc == NRT_OK && n_rays > 0) {
+    PathQueues q;
+    q.org_tmin[0] = static_cast<float4 *>(const_cast<void *>(d_org_tmin));
+    q.dir_tmax[0] = static_cast<float4 *>(const_cast<void *>(d_dir_tmax));
+    q.path_id[0] = const_cast<uint32_t *>(d_path_id);
+    q.org_tmin[1] = static_cast<float4 *>(d_out_org_tmin);
+    q.dir_tmax[1] = static_cast<float4 *>(d_out_dir_tmax);
+    q.path_id[1] = d_out_path_id;
+    q.sh_org_tmin = static_cast<float4 *>(d_sh_org_tmin);
+    q.sh_dir_tmax = static_cast<float4 *>(d_sh_dir_tmax);
+    q.sh_contrib_pix = static_cast<float4 *>(d_sh_contrib_pix);
+    q.weight = static_cast<float4 *>(d_weight);
+    unsigned long long out[3] = {0, 0, 0};
+    rc = scene_path_bounce(c, 0ull, bounce, (uint32_t)n_rays, q, 0, d_accum_rgb, !skip_shadow_pass, out, st);
+    if (rc == NRT_OK) {
+      if (n_continue) *n_continue = out[0];
+      if (n_shadow) *n_shadow = out[1];
+    }
+  }
+  const cudaError_t e = cudaStreamSynchronize(st);  // the call's buffers are freed on return
+  if (rc != NRT_OK) return rc;
+  NRT_CUDA(e);
   return NRT_OK;
 }
