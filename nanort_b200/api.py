@@ -64,6 +64,9 @@ EXPORTS = [
 # every symbol include/nanort_b200_scene_path.h declares (the path tracer over two-level scenes)
 SCENE_PATH_EXPORTS = ["nrt_scene_render_path_device", "nrt_scene_path_bounce_device"]
 
+# every symbol include/nanort_b200_bake.h declares (texel cast and AO bake of UV atlases)
+BAKE_EXPORTS = ["nrt_uv_raster_device", "nrt_bake_ao_device", "nrt_bake_ao_rays_device"]
+
 
 class NanortB200Error(RuntimeError):
     pass
@@ -120,6 +123,35 @@ class PathResult(C.Structure):
     ]
 
 
+class UvRasterParams(C.Structure):
+    """nrt_uv_raster_params: texel grid, uv_region (left, right, top, bottom), texel_offset, flips, TRAVERSE_* flags."""
+    _fields_ = [
+        ("width", C.c_uint32), ("height", C.c_uint32),
+        ("uv_region", C.c_float * 4), ("texel_offset", C.c_float * 2),
+        ("flip_x", C.c_uint32), ("flip_y", C.c_uint32),
+        ("flags", C.c_uint32),
+    ]
+
+
+class BakeParams(C.Structure):
+    """nrt_bake_params: the records' size, samples, AO ray range, TRAVERSE_* flags, optional face-varying normals."""
+    _fields_ = [
+        ("width", C.c_uint32), ("height", C.c_uint32),
+        ("spp", C.c_uint32), ("sample0", C.c_uint32), ("seed", C.c_uint32),
+        ("ao_min_t", C.c_float), ("ao_max_t", C.c_float),
+        ("flags", C.c_uint32),
+        ("d_facevarying_normals", C.c_void_p),
+    ]
+
+
+class BakeResult(C.Structure):
+    _fields_ = [
+        ("texels", C.c_uint64), ("ao_rays", C.c_uint64), ("ao_hits", C.c_uint64),
+        ("traverse_ms", C.c_float), ("total_ms", C.c_float),
+        ("launches", C.c_uint32), ("traverse_launches", C.c_uint32),
+    ]
+
+
 _lib = None
 
 
@@ -169,6 +201,9 @@ def lib():
     L.nrt_scene_render_path_device.argtypes = [vp, C.POINTER(PathParams), vp, vp, C.POINTER(PathResult), vp]
     L.nrt_scene_path_bounce_device.argtypes = [vp, C.POINTER(PathParams), vp, u32, C.c_uint64] + [vp] * 11 + [u64p, u64p,
                                                                                                     C.c_int, vp]
+    L.nrt_uv_raster_device.argtypes = [vp, vp, C.POINTER(UvRasterParams), vp, vp, vp, vp, u64p, vp]
+    L.nrt_bake_ao_device.argtypes = [vp, vp, C.POINTER(BakeParams), vp, C.POINTER(BakeResult), vp]
+    L.nrt_bake_ao_rays_device.argtypes = [vp, vp, C.POINTER(BakeParams), vp, C.c_uint64, u64p, vp]
     L.nrt_build_f64.argtypes = [vp, sz, sz, vp, u32, vp, C.POINTER(vp)]
     L.nrt_build_f64_ex.argtypes = [vp, sz, sz, vp, u32, vp, u32, C.POINTER(vp)]
     L.nrt_adopt_f64.argtypes = [vp, sz, vp, sz, vp, sz, sz, vp, u32, C.POINTER(vp)]
@@ -531,6 +566,37 @@ class BVHAccel:
                                           C.byref(res) if want_result else None,
                                           C.c_void_p(stream) if stream else None))
         return res
+
+    # -- texture-space baking (include/nanort_b200_bake.h)
+    def UVRaster(self, params: UvRasterParams, d_records_ptr, world: "BVHAccel | None" = None, d_position_ptr=None,
+                 d_normal_ptr=None, d_facevarying_normals_ptr=None, stream=None):
+        """The reference uv_raster's texel cast over this accel, built over the UV mesh (nrt_uv_raster_device): writes
+        width * height hit records (HIT_DTYPE) and, with the `world` accel, the position / normal AOVs (float3 per
+        texel).  Device pointers are ints.  Returns the number of covered texels (synchronises `stream`)."""
+        n = C.c_uint64(0)
+        vp = C.c_void_p
+        _check(lib().nrt_uv_raster_device(self._h, world._h if world is not None else None, C.byref(params),
+                                          vp(d_records_ptr), vp(d_position_ptr) if d_position_ptr else None,
+                                          vp(d_normal_ptr) if d_normal_ptr else None,
+                                          vp(d_facevarying_normals_ptr) if d_facevarying_normals_ptr else None,
+                                          C.byref(n), vp(stream) if stream else None))
+        return int(n.value)
+
+    def BakeAO(self, d_records_ptr, params: BakeParams, d_accum_ptr, stream=None, want_result=True):
+        """Cosine AO from every covered texel of UVRaster's records, traced against this (world) accel
+        (nrt_bake_ao_device): d_accum[texel] += 1 per unoccluded ray.  Ordered on the device with the accel's AO and
+        path passes, like RenderAO."""
+        res = BakeResult()
+        _check(lib().nrt_bake_ao_device(self._h, C.c_void_p(d_records_ptr), C.byref(params), C.c_void_p(d_accum_ptr),
+                                        C.byref(res) if want_result else None, C.c_void_p(stream) if stream else None))
+        return res if want_result else None
+
+    def ExportBakeRays(self, d_records_ptr, params: BakeParams, d_rays_ptr, capacity, stream=None):
+        """BakeAO's rays as 36-byte records in slot order (nrt_bake_ao_rays_device); returns their count."""
+        n = C.c_uint64(0)
+        _check(lib().nrt_bake_ao_rays_device(self._h, C.c_void_p(d_records_ptr), C.byref(params), C.c_void_p(d_rays_ptr),
+                                             int(capacity), C.byref(n), C.c_void_p(stream) if stream else None))
+        return int(n.value)
 
 
 # ------------------------------------------------------------------ two-level scene (examples/nanosg)

@@ -255,6 +255,8 @@ struct RecordOnExit {
   cudaStream_t s;
   ~RecordOnExit() { cudaEventRecord(e, s); }
 };
+// render.cu: derives Accel::d_face_n on `s` the first time a pass needs it (call under host_mu, inside the pass)
+int ensure_face_normals(Accel *a, cudaStream_t s);
 // the pass scratch grows only after the pass that last used it has finished
 inline int grow_wave(Accel *a, size_t need) {
   if (a->wave_bytes >= need) return NRT_OK;

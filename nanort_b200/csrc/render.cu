@@ -201,11 +201,7 @@ static int run_ao_pass(const nrt_accel *h, const nrt_ao_params *pp, float *d_acc
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (const int rc = wait_previous_pass(a, s)) return rc;
   const RecordOnExit pass_done{a->pass_done, s};
-  if (!a->d_face_n) {
-    NRT_CUDA(cudaMalloc(&a->d_face_n, sizeof(float4) * (size_t)a->n_prims));
-    face_normals_kernel<<<(a->n_prims + 255) / 256, 256, 0, s>>>(a->d_verts, a->d_faces, a->n_prims, a->d_face_n);
-    NRT_CUDA(cudaGetLastError());
-  }
+  if (const int rc = ensure_face_normals(a, s)) return rc;
   const uint32_t tiles_x = (p.width + p.tile_w - 1) / p.tile_w, tiles_y = (p.height + p.tile_h - 1) / p.tile_h;
   const uint32_t n_tiles = tiles_x * tiles_y;
   const uint32_t my_tiles = n_tiles > p.shard ? (n_tiles - p.shard + p.n_shards - 1) / p.n_shards : 0;
@@ -376,6 +372,14 @@ static int run_ao_pass(const nrt_accel *h, const nrt_ao_params *pp, float *d_acc
 }
 
 namespace nrt {
+int ensure_face_normals(Accel *a, cudaStream_t s) {
+  if (a->d_face_n) return NRT_OK;
+  NRT_CUDA(cudaMalloc(&a->d_face_n, sizeof(float4) * (size_t)a->n_prims));
+  face_normals_kernel<<<(a->n_prims + 255) / 256, 256, 0, s>>>(a->d_verts, a->d_faces, a->n_prims, a->d_face_n);
+  NRT_CUDA(cudaGetLastError());
+  return NRT_OK;
+}
+
 int run_ao_pass_internal(const nrt_accel *h, const nrt_ao_params *pp, float *d_accum, nrt_ao_result *res, void *stream) {
   return run_ao_pass(h, pp, d_accum, res, stream, nullptr, nullptr, nullptr);
 }

@@ -390,6 +390,29 @@ int launch_traverse_path_shadow(const Accel *a, const PathQueues &q, const unsig
                                                                   epi, opt, flags, s);
 }
 
+// Texel cast (bake.cu): the production walk stores each texel's record through its payload; the conformance walk
+// writes records by ray index to d_by_ray, which the caller scatters to the flipped texels.
+int launch_traverse_texels(const Accel *a, const TexelRays &rays, size_t n, const TexelStore &store, Hit16 *d_by_ray,
+                           uint32_t flags, cudaStream_t s) {
+  if (n == 0) return NRT_OK;
+  const TraceOptions16 opt = default_trace_options();
+  if (flags & NRT_TRAVERSE_CONFORMANCE)
+    return launch_conf<TexelRays, false>(a, rays, n, d_by_ray, nullptr, opt, flags, nullptr, s);
+  return launch_fast3_coherent<TexelRays, false>(a, rays, n, TexelStoreEpilogue{store}, opt, flags, nullptr, nullptr, s);
+}
+
+// AO rays of the bake, generated at fetch
+int launch_traverse_bake(const Accel *a, const BakeAoRays &rays, size_t n, float *d_accum, unsigned long long *d_occluded,
+                         uint32_t flags, cudaStream_t s) {
+  if (n == 0) return NRT_OK;
+  const TraceOptions16 opt = default_trace_options();
+  const BakeAccumulateEpilogue epi{d_accum, d_occluded};
+  if (flags & NRT_TRAVERSE_ANY_HIT)
+    return launch_fast3_any<BakeAoRays, false, IncoherentPolicy>(a, rays, n, AnyHit<BakeAccumulateEpilogue>(epi), opt,
+                                                                 flags, nullptr, nullptr, s);
+  return launch_fast3_any<BakeAoRays, false, IncoherentPolicy>(a, rays, n, epi, opt, flags, nullptr, nullptr, s);
+}
+
 int launch_traverse_count(const Accel *a, const Ray36 *d_rays, size_t n, const TraceOptions16 &opt,
                           uint32_t flags, uint64_t *d_counts2, cudaStream_t s) {
   if (a->prim_kind != 0) {  // both counting walks test triangles: their counts would mean nothing on other kinds

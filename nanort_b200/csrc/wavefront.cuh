@@ -252,6 +252,27 @@ __device__ __forceinline__ void geometric_normal(const float *__restrict__ verts
   nz *= il;
 }
 
+// Unit cosine-distributed AO direction about the unit normal n for (pixel or texel, sample): branch-free orthonormal
+// basis around n, then the cosine direction from the random dimensions 2 and 3, normalised (main.cc:216-250).  The AO
+// spawn and the texel bake both take it.
+__device__ __forceinline__ void ao_direction(float nx, float ny, float nz, uint32_t pix, uint32_t smp, uint32_t seed,
+                                             float &ox, float &oy, float &oz) {
+  const float sg = nz >= 0.0f ? 1.0f : -1.0f;
+  const float a = -1.0f / (sg + nz), b = nx * ny * a;
+  const float t1x = 1.0f + sg * nx * nx * a, t1y = sg * b, t1z = -sg * nx;
+  const float t2x = b, t2y = sg + ny * ny * a, t2z = -ny;
+  const float u1 = rand_ps(pix, smp, 2, seed), u2 = rand_ps(pix, smp, 3, seed);
+  const float r = sqrtf(u1), ph = 6.28318530718f * u2;
+  float sn, cs;
+  sincosf(ph, &sn, &cs);
+  const float lx = r * cs, ly = r * sn, lz = sqrtf(fmaxf(0.0f, 1.0f - u1));
+  const float wx = t1x * lx + t2x * ly + nx * lz, wy = t1y * lx + t2y * ly + ny * lz, wz = t1z * lx + t2z * ly + nz * lz;
+  const float il = 1.0f / sqrtf(wx * wx + wy * wy + wz * wz);
+  ox = wx * il;
+  oy = wy * il;
+  oz = wz * il;
+}
+
 // One cosine-hemisphere AO ray from a primary hit.  normals[prim]: geometric_normal() of the primitive, computed once
 // per accel (Accel::d_face_n), so that the spawn needs one 128-bit load instead of two dependent rounds of gathers.
 __device__ __forceinline__ void make_ao_ray(const nrt_ao_params &p, uint32_t pix, uint32_t smp, float4 o, float4 d,
@@ -265,20 +286,10 @@ __device__ __forceinline__ void make_ao_ray(const nrt_ao_params &p, uint32_t pix
     ny = -ny;
     nz = -nz;
   }
-  // branch-free orthonormal basis around n
-  const float sg = nz >= 0.0f ? 1.0f : -1.0f;
-  const float a = -1.0f / (sg + nz), b = nx * ny * a;
-  const float t1x = 1.0f + sg * nx * nx * a, t1y = sg * b, t1z = -sg * nx;
-  const float t2x = b, t2y = sg + ny * ny * a, t2z = -ny;
-  const float u1 = rand_ps(pix, smp, 2, p.seed), u2 = rand_ps(pix, smp, 3, p.seed);
-  const float r = sqrtf(u1), ph = 6.28318530718f * u2;
-  float sn, cs;
-  sincosf(ph, &sn, &cs);
-  const float lx = r * cs, ly = r * sn, lz = sqrtf(fmaxf(0.0f, 1.0f - u1));
-  const float wx = t1x * lx + t2x * ly + nx * lz, wy = t1y * lx + t2y * ly + ny * lz, wz = t1z * lx + t2z * ly + nz * lz;
-  const float il = 1.0f / sqrtf(wx * wx + wy * wy + wz * wz);
+  float wx, wy, wz;
+  ao_direction(nx, ny, nz, pix, smp, p.seed, wx, wy, wz);
   o4 = make_float4(Px, Py, Pz, p.ao_min_t);
-  d4 = make_float4(wx * il, wy * il, wz * il, p.ao_max_t);
+  d4 = make_float4(wx, wy, wz, p.ao_max_t);
 }
 
 // ---- retire-step functors of traverse_fast3_kernel.  Called by ALL 32 lanes of a warp (`retiring` says
@@ -360,6 +371,153 @@ struct AoAccumulateEpilogue {
     if (retiring && !occluded) atomicAdd(accum + ao_pix[ray_idx], 1.0f);
     const unsigned m = __ballot_sync(0xFFFFFFFFu, occluded);
     if (m != 0u && (int)(threadIdx.x & 31) == __ffs(m) - 1) atomicAdd(totals + 1, (unsigned long long)__popc(m));
+  }
+};
+
+// ------------------------------------------------------------------ texture-space baking (bake.cu)
+// Texel cast of the reference's uv_raster (examples/uv_raster/main.cc:752-770): ray i is texel (i % width, i / width),
+// generated at fetch.  Payload: the texel its record goes to, after the flips (main.cc:779-782).
+struct TexelRays {
+  static constexpr int kPayloadWords = 1;
+  static constexpr bool kSharedOrigin = false;
+  FastDiv width;
+  uint32_t height, flip_x, flip_y;
+  float r0, r2, usize, vsize, off0, off1, fw, fh;
+  __device__ __forceinline__ void load(size_t i, float &ox, float &oy, float &oz, float &dx, float &dy, float &dz,
+                                       float &tmin, float &tmax, uint32_t *payload = nullptr) const {
+    uint32_t y, x;
+    width.divmod((uint32_t)i, y, x);
+    ox = r0 + ((float)x * usize + off0) / fw;
+    oy = r2 + ((float)y * vsize + off1) / fh;
+    oz = 1.0f;
+    dx = 0.0f;
+    dy = 0.0f;
+    dz = -1.0f;
+    tmin = 0.0f;
+    tmax = 1.0e30f;
+    if (payload) payload[0] = dest(x, y);
+  }
+  __device__ __forceinline__ uint32_t dest(uint32_t x, uint32_t y) const {
+    const uint32_t px = flip_x ? width.d - 1u - x : x, py = flip_y ? height - 1u - y : y;
+    return py * width.d + px;
+  }
+};
+
+// (1 - u - v) a + u b + v c of three float3 at a, b, c (uv_raster's Lerp, main.cc:58-60)
+__device__ __forceinline__ void lerp3(const float *a, const float *b, const float *c, float u, float v, float &x,
+                                      float &y, float &z) {
+  const float w = 1.0f - u - v;
+  x = w * a[0] + u * b[0] + v * c[0];
+  y = w * a[1] + u * b[1] + v * c[1];
+  z = w * a[2] + u * b[2] + v * c[2];
+}
+
+// What a texel keeps of its cast: the nanort hit record and, with a world mesh, the position and normal AOVs
+// (main.cc:786-829; zeros on an empty texel).  Counts covered texels with one atomic per warp; called by all 32 lanes.
+struct TexelStore {
+  Hit16 *records;
+  float *position, *normal;  // float3 per texel, or nullptr
+  const float *verts;        // world mesh (packed float3) and faces, when an AOV is wanted
+  const uint32_t *faces;
+  const float *fv_normals;  // float[9] per face, for `normal`
+  unsigned long long *covered;
+  __device__ __forceinline__ void operator()(bool active, uint32_t texel, float t, float u, float v, uint32_t prim,
+                                             float max_t) const {
+    const bool hit = active && t < max_t;
+    if (active) {
+      const float4 r = hit ? make_float4(u, v, t, __uint_as_float(prim))
+                           : make_float4(0.0f, 0.0f, 1.0e30f, __uint_as_float(0xFFFFFFFFu));
+      reinterpret_cast<float4 *>(records)[texel] = r;
+      float px = 0.0f, py = 0.0f, pz = 0.0f;
+      if (position) {
+        if (hit) {
+          const uint32_t *f = faces + 3 * (size_t)prim;
+          lerp3(verts + 3 * (size_t)f[0], verts + 3 * (size_t)f[1], verts + 3 * (size_t)f[2], u, v, px, py, pz);
+        }
+        position[3 * (size_t)texel + 0] = px;
+        position[3 * (size_t)texel + 1] = py;
+        position[3 * (size_t)texel + 2] = pz;
+      }
+      if (normal) {
+        px = py = pz = 0.0f;
+        if (hit) {
+          const float *n = fv_normals + 9 * (size_t)prim;
+          lerp3(n, n + 3, n + 6, u, v, px, py, pz);
+        }
+        normal[3 * (size_t)texel + 0] = px;
+        normal[3 * (size_t)texel + 1] = py;
+        normal[3 * (size_t)texel + 2] = pz;
+      }
+    }
+    const unsigned m = __ballot_sync(0xFFFFFFFFu, hit);
+    if (m != 0u && (int)(threadIdx.x & 31) == __ffs(m) - 1) atomicAdd(covered, (unsigned long long)__popc(m));
+  }
+};
+
+struct TexelStoreEpilogue {
+  static constexpr bool kAnyHit = false;
+  TexelStore store;
+  __device__ __forceinline__ void operator()(bool retiring, size_t, float t, float u, float v, uint32_t prim,
+                                             float max_t, const uint32_t *payload) const {
+    store(retiring, payload[0], t, u, v, prim, max_t);
+  }
+};
+
+// AO rays of the bake: slot i of a launch is sample sample0 + i / n_cov of covered texel texels[i % n_cov], with the
+// texel's record (nrt_uv_raster_device) giving the world triangle and the barycentrics.  Payload: the texel.
+struct BakeAoRays {
+  static constexpr int kPayloadWords = 1;
+  static constexpr bool kSharedOrigin = false;
+  const uint32_t *texels;  // covered texels, ascending
+  const float4 *records;   // Hit16 per texel
+  const float *verts;
+  const uint32_t *faces;
+  const float4 *face_n;      // Accel::d_face_n
+  const float *fv_normals;   // float[9] per face, or nullptr
+  FastDiv n_cov;
+  uint32_t sample0, seed;
+  float min_t, max_t;
+  __device__ __forceinline__ void load(size_t i, float &ox, float &oy, float &oz, float &dx, float &dy, float &dz,
+                                       float &tmin, float &tmax, uint32_t *payload) const {
+    uint32_t s, k;
+    n_cov.divmod((uint32_t)i, s, k);
+    const uint32_t texel = __ldg(texels + k), smp = sample0 + s;
+    const float4 r = __ldg(records + texel);
+    const float u = r.x, v = r.y;
+    const uint32_t prim = __float_as_uint(r.w);
+    const uint32_t *f = faces + 3 * (size_t)prim;
+    lerp3(verts + 3 * (size_t)__ldg(f), verts + 3 * (size_t)__ldg(f + 1), verts + 3 * (size_t)__ldg(f + 2), u, v, ox,
+          oy, oz);
+    const float4 n = __ldg(face_n + prim);
+    float nx = n.x, ny = n.y, nz = n.z;
+    if (fv_normals) {  // the geometric normal, on the side of the interpolated shading normal
+      const float *fn = fv_normals + 9 * (size_t)prim;
+      float sx, sy, sz;
+      lerp3(fn, fn + 3, fn + 6, u, v, sx, sy, sz);
+      if (nx * sx + ny * sy + nz * sz < 0.0f) {
+        nx = -nx;
+        ny = -ny;
+        nz = -nz;
+      }
+    }
+    ao_direction(nx, ny, nz, texel, smp, seed, dx, dy, dz);
+    tmin = min_t;
+    tmax = max_t;
+    payload[0] = texel;
+  }
+};
+
+// A bake AO ray: an unoccluded one adds 1 to its texel; occluded ones are counted (one atomic per warp)
+struct BakeAccumulateEpilogue {
+  static constexpr bool kAnyHit = false;
+  float *accum;
+  unsigned long long *occluded;
+  __device__ __forceinline__ void operator()(bool retiring, size_t, float t, float, float, uint32_t, float max_t,
+                                             const uint32_t *payload) const {
+    const bool hit = retiring && (t < max_t);
+    if (retiring && !hit) atomicAdd(accum + payload[0], 1.0f);
+    const unsigned m = __ballot_sync(0xFFFFFFFFu, hit);
+    if (m != 0u && (int)(threadIdx.x & 31) == __ffs(m) - 1) atomicAdd(occluded, (unsigned long long)__popc(m));
   }
 };
 

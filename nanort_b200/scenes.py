@@ -354,6 +354,39 @@ def make_scene(name: str, **kw):
     return np.ascontiguousarray(v, np.float32), np.ascontiguousarray(f, np.uint32)
 
 
+# ----------------------------------------------------------------------------- UV atlases (texel cast / bake)
+# A UV mesh in the layout of the reference's uv_raster (SetupVerticesForUVRaster, examples/uv_raster/main.cc:236-254):
+# vertex 3i + k = (u, v, 0) of corner k of face i, face i = (3i, 3i+1, 3i+2).
+def _uv_mesh(uv):
+    uv = np.asarray(uv, np.float32).reshape(-1, 3, 2)
+    verts = np.zeros((uv.shape[0] * 3, 3), np.float32)
+    verts[:, :2] = uv.reshape(-1, 2)
+    return verts, np.arange(uv.shape[0] * 3, dtype=np.uint32).reshape(-1, 3)
+
+
+def planar_uv(verts, faces):
+    """Face-varying UVs of a heightfield such as terrain(): each corner's (x, z) normalised to [0, 1].  Returns the UV
+    mesh (verts [3n, 3], faces [n, 3])."""
+    v = np.asarray(verts, np.float64)
+    lo, hi = v.min(axis=0), v.max(axis=0)
+    xz = (v[:, [0, 2]] - lo[[0, 2]]) / np.maximum(hi[[0, 2]] - lo[[0, 2]], 1e-30)
+    return _uv_mesh(xz[np.asarray(faces)])
+
+
+def per_face_atlas(n_faces, gutter=0.15):
+    """One right-triangle chart per face for meshes without UVs: faces fill a cols x cols grid of cells (cols =
+    ceil(sqrt(n_faces))), row-major from (0, 0); face i covers the lower-left half of its cell, inset by `gutter`
+    times the cell size, so that no two charts touch.  Returns the UV mesh (verts [3n, 3], faces [n, 3])."""
+    cols = max(1, int(np.ceil(np.sqrt(n_faces))))
+    cell = 1.0 / cols
+    i = np.arange(n_faces)
+    x0 = (i % cols) * cell + gutter * cell
+    y0 = (i // cols) * cell + gutter * cell
+    e = cell * (1.0 - 2.0 * gutter)
+    uv = np.stack([np.stack([x0, y0], 1), np.stack([x0 + e, y0], 1), np.stack([x0, y0 + e], 1)], axis=1)
+    return _uv_mesh(uv)
+
+
 # ----------------------------------------------------------------------------- rays
 def primary_rays(cam, width, height, spp=1, seed=1, pixels=None, sample0=0, min_t=1e-3, max_t=1e30):
     """Jittered pinhole rays, ray index = (pixel * spp + s).  `pixels` optionally restricts to a
