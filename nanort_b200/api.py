@@ -67,6 +67,9 @@ SCENE_PATH_EXPORTS = ["nrt_scene_render_path_device", "nrt_scene_path_bounce_dev
 # every symbol include/nanort_b200_bake.h declares (texel cast and AO bake of UV atlases)
 BAKE_EXPORTS = ["nrt_uv_raster_device", "nrt_bake_ao_device", "nrt_bake_ao_rays_device"]
 
+# every symbol include/nanort_b200_bdpt.h declares (the bidirectional path tracer)
+BDPT_EXPORTS = ["nrt_render_bdpt_device", "nrt_bdpt_export_device"]
+
 
 class NanortB200Error(RuntimeError):
     pass
@@ -152,6 +155,46 @@ class BakeResult(C.Structure):
     ]
 
 
+class BdptParams(C.Structure):
+    """nrt_bdpt_params: camera {org, right, up, forward}, image, samples sample0 .. sample0+spp-1 of spp_total, the path
+    pass's tile map, max_bounces, materials (16 floats each), material ids and face-varying normals (device pointers),
+    flags 0 or TRAVERSE_CONFORMANCE."""
+    _fields_ = [
+        ("cam", C.c_float * 12),
+        ("width", C.c_uint32), ("height", C.c_uint32),
+        ("spp", C.c_uint32), ("sample0", C.c_uint32), ("spp_total", C.c_uint32),
+        ("tile_w", C.c_uint32), ("tile_h", C.c_uint32), ("shard", C.c_uint32), ("n_shards", C.c_uint32),
+        ("max_bounces", C.c_uint32), ("n_materials", C.c_uint32),
+        ("d_materials", C.c_void_p), ("d_material_ids", C.c_void_p), ("d_facevarying_normals", C.c_void_p),
+        ("flags", C.c_uint32), ("pad", C.c_uint32),
+    ]
+
+
+class BdptResult(C.Structure):
+    _fields_ = [
+        ("eye_rays", C.c_uint64), ("light_rays", C.c_uint64), ("connection_rays", C.c_uint64),
+        ("traverse_ms", C.c_float), ("total_ms", C.c_float),
+        ("launches", C.c_uint32), ("traverse_launches", C.c_uint32),
+    ]
+
+
+# nrt_bdpt_vertex: the reference's Vertex (examples/bidir_path_tracer/main.cc:613-622) with its material as an index
+BDPT_LIGHT, BDPT_LENS, BDPT_SURFACE = 0, 1, 2
+BDPT_VERTEX_DTYPE = np.dtype([
+    ("position", "<f4", (3,)), ("original_norm", "<f4", (3,)), ("norm", "<f4", (3,)), ("beta", "<f4", (3,)),
+    ("wo", "<f4", (3,)), ("pdf_fwd", "<f4"), ("pdf_rev", "<f4"), ("type", "<u4"), ("material", "<u4"),
+    ("prim_id", "<u4"),
+])
+assert BDPT_VERTEX_DTYPE.itemsize == 80
+
+
+def bdpt_slots(params: "BdptParams") -> int:
+    """Slots of one nrt_bdpt_export_device call: this shard's tiles x tile_w x tile_h x spp."""
+    tiles = -(-params.width // params.tile_w) * -(-params.height // params.tile_h)
+    mine = (tiles - params.shard + params.n_shards - 1) // params.n_shards if tiles > params.shard else 0
+    return mine * params.tile_w * params.tile_h * params.spp
+
+
 _lib = None
 
 
@@ -204,6 +247,8 @@ def lib():
     L.nrt_uv_raster_device.argtypes = [vp, vp, C.POINTER(UvRasterParams), vp, vp, vp, vp, u64p, vp]
     L.nrt_bake_ao_device.argtypes = [vp, vp, C.POINTER(BakeParams), vp, C.POINTER(BakeResult), vp]
     L.nrt_bake_ao_rays_device.argtypes = [vp, vp, C.POINTER(BakeParams), vp, C.c_uint64, u64p, vp]
+    L.nrt_render_bdpt_device.argtypes = [vp, C.POINTER(BdptParams), vp, C.POINTER(BdptResult), vp]
+    L.nrt_bdpt_export_device.argtypes = [vp, C.POINTER(BdptParams), vp, vp, vp, vp, vp, C.POINTER(BdptResult), vp]
     L.nrt_build_f64.argtypes = [vp, sz, sz, vp, u32, vp, C.POINTER(vp)]
     L.nrt_build_f64_ex.argtypes = [vp, sz, sz, vp, u32, vp, u32, C.POINTER(vp)]
     L.nrt_adopt_f64.argtypes = [vp, sz, vp, sz, vp, sz, sz, vp, u32, C.POINTER(vp)]
@@ -597,6 +642,27 @@ class BVHAccel:
         _check(lib().nrt_bake_ao_rays_device(self._h, C.c_void_p(d_records_ptr), C.byref(params), C.c_void_p(d_rays_ptr),
                                              int(capacity), C.byref(n), C.c_void_p(stream) if stream else None))
         return int(n.value)
+
+    def RenderBDPT(self, params: BdptParams, d_accum_rgb_ptr, stream=None, want_result=True):
+        """The reference's bidirectional path tracer (nrt_render_bdpt_device): each sample's connectPath colour is
+        added to d_accum_rgb (float[3 * width * height]), each pixel's samples in ascending order.  Ordered on the
+        device with the accel's other passes, like RenderPath."""
+        res = BdptResult()
+        _check(lib().nrt_render_bdpt_device(self._h, C.byref(params), C.c_void_p(d_accum_rgb_ptr),
+                                            C.byref(res) if want_result else None,
+                                            C.c_void_p(stream) if stream else None))
+        return res if want_result else None
+
+    def ExportBDPT(self, params: BdptParams, d_eye_ptr, d_light_ptr, d_n_eye_ptr, d_n_light_ptr, d_sample_rgb_ptr,
+                   stream=None):
+        """RenderBDPT's samples, per slot (nrt_bdpt_export_device): both subpaths (BDPT_VERTEX_DTYPE records,
+        max_bounces + 1 per slot), their lengths (uint32) and the colour (float[3]); bdpt_slots(params) slots."""
+        res = BdptResult()
+        _check(lib().nrt_bdpt_export_device(self._h, C.byref(params), C.c_void_p(d_eye_ptr), C.c_void_p(d_light_ptr),
+                                            C.c_void_p(d_n_eye_ptr), C.c_void_p(d_n_light_ptr),
+                                            C.c_void_p(d_sample_rgb_ptr), C.byref(res),
+                                            C.c_void_p(stream) if stream else None))
+        return res
 
 
 # ------------------------------------------------------------------ two-level scene (examples/nanosg)

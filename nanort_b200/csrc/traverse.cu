@@ -413,6 +413,59 @@ int launch_traverse_bake(const Accel *a, const BakeAoRays &rays, size_t n, float
   return launch_fast3_any<BakeAoRays, false, IncoherentPolicy>(a, rays, n, epi, opt, flags, nullptr, nullptr, s);
 }
 
+// The conformance walk with a retire step: the reference-order walk of traverse_conformance_kernel, then the
+// epilogue, called by every lane of the block (lanes past n retire nothing).
+template <class Rays, class Epi>
+__global__ void __launch_bounds__(128)
+    traverse_conformance_epi_kernel(const Node40 *__restrict__ nodes, const PackedTri *__restrict__ tris, Rays rays,
+                                    size_t n, Epi epi, TraceOptions16 opt, uint32_t flags,
+                                    const unsigned long long *n_ptr) {
+  if (n_ptr) n = (size_t)*n_ptr;
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  Best best;
+  best.t = 0.0f;
+  best.u = 0.0f;
+  best.v = 0.0f;
+  best.prim = 0xFFFFFFFFu;
+  float max_t = 0.0f;
+  if (i < n) {
+    float ox, oy, oz, dx, dy, dz, min_t;
+    rays.load(i, ox, oy, oz, dx, dy, dz, min_t, max_t);
+    RayCtx c;
+    setup_ray(c, ox, oy, oz, dx, dy, dz, min_t, (flags & NRT_TRAVERSE_CPP03_INVERSE) != 0);
+    best.t = max_t;
+    reference_walk(nodes, c, min_t, max_t, PackedTriLeaf{tris, c, opt, best});
+  }
+  epi(i < n, i, best.t, best.u, best.v, best.prim, max_t, nullptr);
+}
+
+template <class Rays, class Epi, class P>
+static int launch_bdpt(const Accel *a, const Rays &rays, const Epi &epi, const unsigned long long *d_count,
+                       size_t capacity, uint32_t flags, cudaStream_t s) {
+  if (capacity == 0) return NRT_OK;
+  const TraceOptions16 opt = default_trace_options();
+  if (flags & NRT_TRAVERSE_CONFORMANCE) {
+    traverse_conformance_epi_kernel<Rays, Epi><<<(unsigned)((capacity + 127) / 128), 128, 0, s>>>(
+        a->d_nodes, a->d_tris, rays, capacity, epi, opt, flags, d_count);
+    NRT_CUDA(cudaGetLastError());
+    return NRT_OK;
+  }
+  return launch_fused<Epi, P, Rays>(a, rays, capacity, d_count, epi, opt, flags, s);
+}
+
+// Bidirectional path tracer (bdpt.cu): subpath bounces, whose retire step is raytrace's per-hit block (the path
+// radiance launch's policy: a shading retire step), and the connection rays, whose retire step is calcG's test
+// (incoherent rays, a light retire step).
+int launch_traverse_bdpt_bounce(const Accel *a, const bd::BounceRays &rays, const bd::BounceEpilogue &epi,
+                                const unsigned long long *d_count, size_t capacity, uint32_t flags, cudaStream_t s) {
+  return launch_bdpt<bd::BounceRays, bd::BounceEpilogue, PathRadiancePolicy>(a, rays, epi, d_count, capacity, flags, s);
+}
+
+int launch_traverse_bdpt_connect(const Accel *a, const bd::ConnRays &rays, const bd::ConnEpilogue &epi,
+                                 const unsigned long long *d_count, size_t capacity, uint32_t flags, cudaStream_t s) {
+  return launch_bdpt<bd::ConnRays, bd::ConnEpilogue, IncoherentPolicy>(a, rays, epi, d_count, capacity, flags, s);
+}
+
 int launch_traverse_count(const Accel *a, const Ray36 *d_rays, size_t n, const TraceOptions16 &opt,
                           uint32_t flags, uint64_t *d_counts2, cudaStream_t s) {
   if (a->prim_kind != 0) {  // both counting walks test triangles: their counts would mean nothing on other kinds

@@ -4,6 +4,7 @@
 //   hit point main.cc:860, geometric normal main.cc:306-312 flipped to the viewer main.cc:878-881,
 //   orthonormal basis + cosine direction main.cc:216-250, occlusion query main.cc:675-701.
 #pragma once
+#include "../../include/nanort_b200_bdpt.h"
 #include "common.cuh"
 
 namespace nrt {
@@ -840,6 +841,411 @@ struct ShadowAccumulateEpilogue {
     }
   }
 };
+
+// ------------------------------------------------------------------ bidirectional path tracing (bdpt.cu)
+// The reference's examples/bidir_path_tracer/main.cc restated in float32 with its operation order (the library is
+// compiled with --fmad=false).  float3 is the reference's float3: `f * v` and `v * f` both round v.x * f, `v / f`
+// divides each component.
+namespace bd {
+
+constexpr float kEps = 0.001f;
+constexpr float kInf = 1.0e30f;
+constexpr float kPi = 3.14159274101257324f;  // 4.0f * std::atan(1.0f)
+constexpr uint32_t kNone = 0xFFFFFFFFu;
+
+__device__ __forceinline__ float3 f3(float x, float y, float z) { return make_float3(x, y, z); }
+__device__ __forceinline__ float3 f3(const float *p) { return make_float3(p[0], p[1], p[2]); }
+__device__ __forceinline__ float3 add(float3 a, float3 b) { return f3(a.x + b.x, a.y + b.y, a.z + b.z); }
+__device__ __forceinline__ float3 sub(float3 a, float3 b) { return f3(a.x - b.x, a.y - b.y, a.z - b.z); }
+__device__ __forceinline__ float3 mul(float3 a, float3 b) { return f3(a.x * b.x, a.y * b.y, a.z * b.z); }
+__device__ __forceinline__ float3 mul(float3 v, float f) { return f3(v.x * f, v.y * f, v.z * f); }
+__device__ __forceinline__ float3 div(float3 v, float f) { return f3(v.x / f, v.y / f, v.z / f); }
+__device__ __forceinline__ float3 neg(float3 v) { return f3(-v.x, -v.y, -v.z); }
+__device__ __forceinline__ float dot(float3 a, float3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
+__device__ __forceinline__ float3 cross(float3 a, float3 b) {
+  return f3(a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x);
+}
+__device__ __forceinline__ float length(float3 v) { return sqrtf(v.x * v.x + v.y * v.y + v.z * v.z); }
+// float3::normalize: the threshold test and 1.0 / len in double (main.cc:218-226)
+__device__ __forceinline__ float3 normalize(float3 v) {
+  const float len = length(v);
+  if (fabs((double)len) > 1.0e-6) {
+    const float inv = (float)(1.0 / (double)len);
+    v = mul(v, inv);
+  }
+  return v;
+}
+__device__ __forceinline__ bool black(float3 v) { return v.x == 0.0f && v.y == 0.0f && v.z == 0.0f; }
+__device__ __forceinline__ float fmax0(float x) { return 0.0f < x ? x : 0.0f; }  // std::max(0.0f, x)
+
+// Random (main.cc:132-157): xorshift128 seeded by the reference's recurrence; nextReal can return 1.0f
+struct Random {
+  uint32_t s[4];
+  __device__ __forceinline__ void seed(uint32_t x) {
+#pragma unroll
+    for (int i = 1; i <= 4; i++) s[i - 1] = x = 1812433253u * (x ^ (x >> 30)) + (uint32_t)i;
+  }
+  __device__ __forceinline__ uint32_t next() {
+    const uint32_t t = s[0] ^ (s[0] << 11);
+    s[0] = s[1];
+    s[1] = s[2];
+    s[2] = s[3];
+    return s[3] = (s[3] ^ (s[3] >> 19)) ^ (t ^ (t >> 8));
+  }
+  __device__ __forceinline__ float real() { return (float)next() / 4294967296.0f; }  // (float)UINT_MAX
+};
+
+__device__ __forceinline__ bool is_delta(const PathMaterial *m) {  // Vertex::isDelta; no material: not delta
+  if (!m) return false;
+  return m->specular[0] != 0.0f || m->specular[1] != 0.0f || m->specular[2] != 0.0f ||
+         m->transmittance[0] != 0.0f || m->transmittance[1] != 0.0f || m->transmittance[2] != 0.0f;
+}
+
+// The Fresnel factor and lobe probabilities shared by Vertex::f, sampleBRDF and pdfBRDF (main.cc:641-665, 782-808,
+// 846-870).  Returns totalrho; the rho are normalised only when it is >= 0.0001f.
+__device__ __forceinline__ float lobes(const PathMaterial &m, float3 wo, float3 on, float3 n, float &rhoS, float &rhoD,
+                                       float &rhoR, float &inside, float &n1) {
+  const float dd = dot(neg(wo), on);
+  inside = dd < 0 ? -1.0f : 1.0f;  // sign()
+  n1 = inside < 0 ? (float)(1.0 / (double)m.ior) : m.ior;
+  const float n2 = (float)(1.0 / (double)n1);
+  const float r0s = (n1 - n2) / (n1 + n2);
+  const float r0 = r0s * r0s;  // fresnel_schlick
+  const float c = 1.0f - dot(wo, n);
+  const float fresnel = r0 + (1.0f - r0) * (c * c * c * c * c);
+  const float3 third = f3(1.0f / 3.0f, 1.0f / 3.0f, 1.0f / 3.0f);
+  rhoS = dot(third, f3(m.specular)) * fresnel;
+  rhoD = (float)((double)dot(third, f3(m.diffuse)) * (1.0 - (double)fresnel) * (1.0 - (double)m.dissolve));
+  rhoR = (float)((double)dot(third, f3(m.transmittance)) * (1.0 - (double)fresnel) * (double)m.dissolve);
+  const float total = rhoS + rhoD + rhoR;
+  if (!(total < 0.0001f)) {
+    rhoS /= total;
+    rhoD /= total;
+    rhoR /= total;
+  }
+  return total;
+}
+
+// Vertex::f (main.cc:634-689) of vertex (p, on, n, wo, material m) towards position q
+__device__ __forceinline__ float3 vertex_f(const nrt_bdpt_vertex &v, const PathMaterial *m, float3 q) {
+  const float3 n = f3(v.norm), wo = f3(v.wo);
+  const float3 wi = sub(q, f3(v.position));
+  const bool refl = dot(wi, n) * dot(wo, n) > 0.0f;
+  const PathMaterial mm = m ? *m : PathMaterial{};
+  float rhoS, rhoD, rhoR, inside, n1;
+  if (lobes(mm, wo, f3(v.original_norm), n, rhoS, rhoD, rhoR, inside, n1) < 0.0001f) return f3(0.0f, 0.0f, 0.0f);
+  float3 ret = f3(0.0f, 0.0f, 0.0f);
+  float weight = 0.0f;
+  if (rhoS > 0.0f && refl) {
+    ret = add(ret, mul(f3(0.0f, 0.0f, 0.0f), rhoS));
+    weight += rhoS;
+  }
+  if (rhoD > 0.0f && refl) {
+    ret = add(ret, div(mul(f3(mm.diffuse), rhoD), kPi));
+    weight += rhoD;
+  }
+  if (rhoR > 0.0f && !refl) {
+    ret = add(ret, mul(f3(0.0f, 0.0f, 0.0f), rhoR));
+    weight += rhoR;
+  }
+  if (weight != 0.0f) ret = div(ret, weight);
+  return ret;
+}
+
+// pdfBRDF (main.cc:839-886); no material: 0
+__device__ __forceinline__ float pdf_brdf(const PathMaterial *m, float3 wi, float3 wo, float3 on, float3 n) {
+  const bool refl = dot(wi, n) * dot(wo, n) > 0.0f;
+  const PathMaterial mm = m ? *m : PathMaterial{};
+  float rhoS, rhoD, rhoR, inside, n1;
+  if (lobes(mm, wo, on, n, rhoS, rhoD, rhoR, inside, n1) < 0.0001f) return 0.0f;
+  float pdf = 0.0f;
+  if (rhoS > 0.0f && refl) pdf += 0.0f;
+  if (rhoD > 0.0f && refl) pdf += rhoD * fabsf(dot(wi, n)) / kPi;
+  if (rhoR > 0.0f && !refl) pdf += 0.0f;
+  return pdf;
+}
+
+// directionCosTheta (main.cc:264-280): 2.0 * kPi * u2, sqrt(u1) and 1.0 - u1 in double; cosf / sinf as the correctly
+// rounded cos / sin of the float phi
+__device__ __forceinline__ float3 direction_cos_theta(float3 n, float u1, float u2, float &pdf) {
+  const float phi = (float)(2.0 * (double)kPi * (double)u2);
+  const float r = (float)sqrt((double)u1);
+  const float x = r * (float)cos((double)phi);
+  const float y = r * (float)sin((double)phi);
+  const float z = sqrtf((float)(1.0 - (double)u1));
+  pdf = z / kPi;
+  float3 xd = fabsf(n.x) < fabsf(n.y) ? f3(1.0f, 0.0f, 0.0f) : f3(0.0f, 1.0f, 0.0f);
+  const float3 yd = normalize(cross(n, xd));
+  xd = cross(yd, n);
+  return add(add(mul(xd, x), mul(yd, y)), mul(n, z));
+}
+
+// sampleBRDF (main.cc:776-837).  The diffuse lobe's directionCosTheta(norm, rng.nextReal(), rng.nextReal(), pdf) draws
+// its arguments right to left, as GCC on x86-64 evaluates them: u2 first.
+__device__ __forceinline__ float3 sample_brdf(const PathMaterial &m, float3 wo, float3 on, float3 n, Random &rng,
+                                              float3 &wi, float &pdf) {
+  float rhoS, rhoD, rhoR, inside, n1;
+  if (lobes(m, wo, on, n, rhoS, rhoD, rhoR, inside, n1) < 0.0001f) {
+    pdf = 0.0f;
+    return f3(0.0f, 0.0f, 0.0f);
+  }
+  float3 f = f3(0.0f, 0.0f, 0.0f);
+  const float rnd = rng.real();
+  pdf = 0.0f;
+  if (rnd < rhoS) {
+    const float3 I = neg(wo);
+    wi = sub(I, mul(n, 2.0f * dot(I, n)));  // reflect
+    const float c = fabsf(dot(wi, n));
+    if (c >= kEps) {
+      pdf = rhoS;
+      f = div(mul(f3(m.specular), rhoS), c);
+    }
+  } else if (rnd < rhoS + rhoD) {
+    const float u2 = rng.real();
+    const float u1 = rng.real();
+    wi = direction_cos_theta(n, u1, u2, pdf);
+    pdf *= rhoD;
+    f = div(mul(f3(m.diffuse), rhoD), kPi);
+  } else if (rnd < rhoD + rhoS + rhoR) {
+    const float3 I = neg(wo), N = mul(on, -inside);  // refract(-wo, -inside * origNorm, n1)
+    const float ndi = dot(N, I);
+    const float k = 1.0f - n1 * n1 * (1.0f - ndi * ndi);
+    wi = k < 0.0f ? f3(0.0f, 0.0f, 0.0f) : sub(mul(I, n1), mul(N, n1 * ndi + sqrtf(k)));
+    const float c = fabsf(dot(wi, n));
+    if (c >= kEps) {
+      pdf = rhoR;
+      f = div(mul(f3(m.transmittance), rhoR), c);
+    }
+  }
+  return f;
+}
+
+// What the stage kernels and retire steps read of the mesh and its lights.
+struct Scene {
+  const PathMaterial *mats;
+  const uint32_t *mat_ids;
+  const float *fv_normals;  // float[9] per face
+  const float *verts;
+  const uint32_t *faces;
+  const float *cdf;          // LightSampler::cdf_
+  const uint32_t *light_ids; // LightSampler::ids_
+  const float *total_area;   // LightSampler::totalArea_ (device scalar)
+  uint32_t n_lights, n_materials;
+  __device__ __forceinline__ const PathMaterial *mat(uint32_t id) const { return id == kNone ? nullptr : mats + id; }
+};
+
+// Per sample: the ray about to be traced and what raytrace keeps between bounces, and the sample's generator
+struct PathState {
+  float4 org_pdf;  // rayOrg, pdfFwd
+  float4 dir;      // rayDir
+  float4 beta;
+  uint4 rng;
+};
+
+// Pass layout of a wave: vertex records of sample `slot` at verts + slot * stride
+struct Subpaths {
+  nrt_bdpt_vertex *eye, *light;
+  uint32_t *n_eye, *n_light;
+  uint32_t stride;  // max_bounces + 1
+};
+
+__device__ __forceinline__ void vstore(nrt_bdpt_vertex &d, float3 p, float3 on, float3 n, float3 beta, float3 wo,
+                                       float pdf_fwd, float pdf_rev, uint32_t type, uint32_t mat, uint32_t prim) {
+  nrt_bdpt_vertex v;
+  v.position[0] = p.x, v.position[1] = p.y, v.position[2] = p.z;
+  v.original_norm[0] = on.x, v.original_norm[1] = on.y, v.original_norm[2] = on.z;
+  v.norm[0] = n.x, v.norm[1] = n.y, v.norm[2] = n.z;
+  v.beta[0] = beta.x, v.beta[1] = beta.y, v.beta[2] = beta.z;
+  v.wo[0] = wo.x, v.wo[1] = wo.y, v.wo[2] = wo.z;
+  v.pdf_fwd = pdf_fwd;
+  v.pdf_rev = pdf_rev;
+  v.type = type;
+  v.material = mat;
+  v.prim_id = prim;
+  d = v;
+}
+
+// raytrace's per-hit block (main.cc:925-1011) for a ray of subpath `verts` (n vertices so far) that hit `prim` at t.
+// Appends the vertex (unless a light subpath hit a light), converts its pdfFwd, samples the BRDF with the sample's
+// generator, writes prev.pdfRev and the next ray into st.  Returns whether the subpath traces another ray.
+__device__ __forceinline__ bool subpath_hit(const Scene &sc, bool eye, uint32_t max_bounces, PathState &st,
+                                            nrt_bdpt_vertex *verts, uint32_t &n, float t, float u, float v,
+                                            uint32_t prim) {
+  const float3 org = f3(st.org_pdf.x, st.org_pdf.y, st.org_pdf.z), dir = f3(st.dir.x, st.dir.y, st.dir.z);
+  float3 beta = f3(st.beta.x, st.beta.y, st.beta.z);
+  const float3 next = add(org, mul(dir, t));
+  const float *fn = sc.fv_normals + 9 * (size_t)prim;
+  const float w = (float)(1.0 - (double)u - (double)v);
+  float3 nrm = normalize(add(add(mul(f3(fn), w), mul(f3(fn + 3), u)), mul(f3(fn + 6), v)));
+  const float3 on = nrm;
+  if (dot(nrm, dir) > 0) nrm = mul(nrm, -1.0f);
+  const uint32_t mid = sc.mat_ids[prim];
+  const PathMaterial m = sc.mats[mid];
+  const bool light = m.emission[0] != 0.0f || m.emission[1] != 0.0f || m.emission[2] != 0.0f;  // isLight
+  if (light && !eye) return false;
+  if (light) beta = mul(mul(beta, f3(m.emission)), fmax0(dot(on, neg(dir))));
+  const nrt_bdpt_vertex prev = verts[n - 1];
+  float3 to = sub(next, f3(prev.position));
+  const float dist = length(to);
+  to = div(to, dist);
+  const float pdf_fwd = st.org_pdf.w * (dot(to, f3(prev.norm)) / (dist * dist));
+  vstore(verts[n], next, on, nrm, beta, normalize(neg(dir)), pdf_fwd, 0.0f, light ? NRT_BDPT_LIGHT : NRT_BDPT_SURFACE,
+         mid, prim);
+  const uint32_t b = n - 1;  // raytrace's loop counter
+  n++;
+  if (light) return false;
+  Random rng;
+  rng.s[0] = st.rng.x, rng.s[1] = st.rng.y, rng.s[2] = st.rng.z, rng.s[3] = st.rng.w;
+  float3 out = f3(0.0f, 0.0f, 0.0f);
+  float pdf;
+  const float3 f = sample_brdf(m, neg(dir), on, nrm, rng, out, pdf);
+  st.rng = make_uint4(rng.s[0], rng.s[1], rng.s[2], rng.s[3]);
+  if (pdf == 0.0f) return false;
+  beta = div(mul(mul(f, beta), fabsf(dot(nrm, out))), pdf);
+  if (black(beta)) return false;
+  const float pdf_rev = pdf_brdf(&m, out, neg(dir), on, nrm);
+  st.org_pdf = make_float4(next.x, next.y, next.z, pdf);
+  st.dir = make_float4(out.x, out.y, out.z, 0.0f);
+  st.beta = make_float4(beta.x, beta.y, beta.z, 0.0f);
+  verts[n - 2].pdf_rev = pdf_rev * fabsf(dot(neg(to), nrm)) / (dist * dist);
+  return b + 1 < max_bounces;
+}
+
+// One connection of connectPath (main.cc:1263-1283): eye vertex e - 1 and light vertex l - 1 of sample `slot`, its
+// unshadowed L and its weightMIS; the retire step of its calcG ray turns L into mis * (L * G).
+struct Conn {
+  uint32_t slot;
+  uint32_t el;  // e | l << 16
+  float L[3];
+  float mis;
+};
+static_assert(sizeof(Conn) == 24, "Conn");
+
+// calcG's ray (main.cc:1215-1227): from the eye vertex towards the light vertex, [kEps, kInf)
+__device__ __forceinline__ void conn_ray(float3 pe, float3 pl, float3 &to, float &dist) {
+  to = sub(pl, pe);
+  dist = length(to);
+  to = div(to, dist);
+}
+
+// calcG's test and cosines (main.cc:1233-1243) from the closest hit at t (hit: t < max_t)
+__device__ __forceinline__ float calc_g(float3 to, float dist, float3 ne, float3 nl, bool hit, float t) {
+  if (!hit) return 0.0f;
+  if (fabsf(dist - t) > kEps) return 0.0f;
+  const float d1 = fmax0(dot(to, ne)), d2 = fmax0(dot(neg(to), nl));
+  return d1 * d2 / (dist * dist);
+}
+
+// Ray loader of the connection launch: the ray is rebuilt from the record's two vertices at fetch
+struct ConnRays {
+  static constexpr int kPayloadWords = 0;
+  static constexpr bool kSharedOrigin = false;
+  const Conn *conns;
+  Subpaths sp;
+  __device__ __forceinline__ void load(size_t i, float &ox, float &oy, float &oz, float &dx, float &dy, float &dz,
+                                       float &tmin, float &tmax, uint32_t * = nullptr) const {
+    const uint32_t slot = __ldg(&conns[i].slot), el = __ldg(&conns[i].el);
+    const float *pe = sp.eye[(size_t)slot * sp.stride + (el & 0xFFFFu) - 1].position;
+    const float *pl = sp.light[(size_t)slot * sp.stride + (el >> 16) - 1].position;
+    float3 to;
+    float dist;
+    conn_ray(f3(pe), f3(pl), to, dist);
+    ox = pe[0];
+    oy = pe[1];
+    oz = pe[2];
+    dx = to.x;
+    dy = to.y;
+    dz = to.z;
+    tmin = kEps;
+    tmax = kInf;
+  }
+};
+
+// Connection retire step: L becomes mis * (L * G) in place
+struct ConnEpilogue {
+  static constexpr bool kAnyHit = false;
+  Conn *conns;
+  Subpaths sp;
+  __device__ __forceinline__ void operator()(bool retiring, size_t ray_idx, float t, float, float, uint32_t,
+                                             float max_t, const uint32_t *) const {
+    if (!retiring) return;
+    Conn &c = conns[ray_idx];
+    const uint32_t slot = c.slot, el = c.el;
+    const nrt_bdpt_vertex &ev = sp.eye[(size_t)slot * sp.stride + (el & 0xFFFFu) - 1];
+    const nrt_bdpt_vertex &lv = sp.light[(size_t)slot * sp.stride + (el >> 16) - 1];
+    float3 to;
+    float dist;
+    conn_ray(f3(ev.position), f3(lv.position), to, dist);
+    const float G = calc_g(to, dist, f3(ev.norm), f3(lv.norm), t < max_t, t);
+    const float mis = c.mis;
+    c.L[0] = (c.L[0] * G) * mis;
+    c.L[1] = (c.L[1] * G) * mis;
+    c.L[2] = (c.L[2] * G) * mis;
+  }
+};
+
+// Ray loader of a subpath bounce: the queued sample's next ray
+struct BounceRays {
+  static constexpr int kPayloadWords = 0;
+  static constexpr bool kSharedOrigin = false;
+  const uint32_t *queue;
+  const PathState *st;
+  __device__ __forceinline__ void load(size_t i, float &ox, float &oy, float &oz, float &dx, float &dy, float &dz,
+                                       float &tmin, float &tmax, uint32_t * = nullptr) const {
+    const uint32_t slot = __ldg(queue + i);
+    const float4 o = __ldg(&st[slot].org_pdf), d = __ldg(&st[slot].dir);
+    ox = o.x;
+    oy = o.y;
+    oz = o.z;
+    dx = d.x;
+    dy = d.y;
+    dz = d.z;
+    tmin = kEps;
+    tmax = kInf;
+  }
+};
+
+// Appends `slot` to a queue, one atomic per warp; called by all 32 lanes
+__device__ __forceinline__ void queue_append(uint32_t *queue, unsigned long long *count, bool put, uint32_t slot) {
+  const unsigned m = __ballot_sync(0xFFFFFFFFu, put);
+  if (m == 0u) return;
+  const int lane = threadIdx.x & 31, leader = __ffs(m) - 1;
+  unsigned long long base = 0;
+  if (lane == leader) base = atomicAdd(count, (unsigned long long)__popc(m));
+  base = __shfl_sync(0xFFFFFFFFu, base, leader);
+  if (put) queue[base + __popc(m & ((1u << lane) - 1u))] = slot;
+}
+
+// Subpath bounce retire step: raytrace's per-hit block; a miss ends the subpath
+struct BounceEpilogue {
+  static constexpr bool kAnyHit = false;
+  Scene sc;
+  Subpaths sp;
+  PathState *st;
+  const uint32_t *queue_in;
+  uint32_t *queue_out;
+  unsigned long long *count_out;
+  uint32_t max_bounces;
+  int eye;
+  __device__ __forceinline__ void operator()(bool retiring, size_t ray_idx, float t, float u, float v, uint32_t prim,
+                                             float max_t, const uint32_t *) const {
+    bool cont = false;
+    uint32_t slot = 0;
+    if (retiring && t < max_t) {
+      slot = queue_in[ray_idx];
+      PathState s = st[slot];
+      uint32_t *np = (eye ? sp.n_eye : sp.n_light) + slot;
+      uint32_t n = *np;
+      cont = subpath_hit(sc, eye != 0, max_bounces, s, (eye ? sp.eye : sp.light) + (size_t)slot * sp.stride, n, t, u,
+                         v, prim);
+      *np = n;
+      st[slot] = s;
+    }
+    queue_append(queue_out, count_out, cont, slot);
+  }
+};
+
+}  // namespace bd
 
 // NRT_TRAVERSE_ANY_HIT: the same retire steps on rays the kernel stops at their first hit
 template <class E>
