@@ -11,10 +11,9 @@ import numpy as np
 import pytest
 
 import bdpt_model as M
+from bdpt_helpers import FIELDS, MB, Setup, _bits, _compare_samples, frame_from_samples, slot_map
 
 pytestmark = pytest.mark.gpu
-
-MB = 10  # the reference's uMaxBounces
 
 
 @pytest.fixture(scope="module")
@@ -26,110 +25,12 @@ def ref_mod():
     return bdpt_ref
 
 
-class Setup:
-    """A mesh with materials on the device and in the reference, with a reference-tree accel and a production one."""
-
-    def __init__(self, ref_mod, v, f, mats, ids):
-        import torch
-
-        from nanort_b200 import api
-
-        self.api = api
-        self.v, self.f = np.ascontiguousarray(v, np.float32), np.ascontiguousarray(f, np.uint32)
-        self.mats = np.ascontiguousarray(np.asarray(mats).view(np.float32).reshape(-1, 16))
-        self.ids = np.ascontiguousarray(ids, np.uint32)
-        self.fvn = M.flat_normals(self.v, self.f)
-        self.ref = ref_mod.BdptReference(self.v, self.f, self.ids, self.mats, self.fvn, api.BDPT_VERTEX_DTYPE)
-        dev = "cuda:0"
-        self.d_mats = torch.from_numpy(self.mats.copy()).to(dev)
-        self.d_ids = torch.from_numpy(self.ids.view(np.int32).copy()).to(dev)
-        self.d_fvn = torch.from_numpy(self.fvn.copy()).to(dev)
-        self.conf = api.BVHAccel(device=0)
-        assert self.conf.Build(len(self.f), self.v, self.f, flags=api.BUILD_REFERENCE_TREE)
-        self.fast = api.BVHAccel(device=0)
-        assert self.fast.Build(len(self.f), self.v, self.f)
-
-    def params(self, W, H, spp, sample0=0, spp_total=None, tile=(16, 8), shard=0, n_shards=1, max_bounces=MB,
-               flags=1, cam=M.REFERENCE_CAMERA):
-        p = self.api.BdptParams()
-        for k in range(12):
-            p.cam[k] = float(cam[k])
-        p.width, p.height, p.spp, p.sample0 = W, H, spp, sample0
-        p.spp_total = spp_total if spp_total is not None else sample0 + spp
-        p.tile_w, p.tile_h, p.shard, p.n_shards = tile[0], tile[1], shard, n_shards
-        p.max_bounces, p.n_materials = max_bounces, len(self.mats)
-        p.d_materials, p.d_material_ids, p.d_facevarying_normals = (self.d_mats.data_ptr(), self.d_ids.data_ptr(),
-                                                                    self.d_fvn.data_ptr())
-        p.flags = flags
-        return p
-
-    def export(self, p, accel=None, stream=None):
-        import torch
-
-        accel = accel or (self.conf if p.flags else self.fast)
-        n = self.api.bdpt_slots(p)
-        rec = p.max_bounces + 1
-        eye = torch.zeros(n * rec * 80, dtype=torch.uint8, device="cuda:0")
-        light = torch.zeros_like(eye)
-        ne = torch.zeros(n, dtype=torch.int32, device="cuda:0")
-        nl = torch.zeros_like(ne)
-        rgb = torch.zeros(3 * n, dtype=torch.float32, device="cuda:0")
-        r = accel.ExportBDPT(p, eye.data_ptr(), light.data_ptr(), ne.data_ptr(), nl.data_ptr(), rgb.data_ptr(), stream)
-        torch.cuda.synchronize()
-        dt = self.api.BDPT_VERTEX_DTYPE
-        return dict(eye=eye.cpu().numpy().view(dt).reshape(n, rec), light=light.cpu().numpy().view(dt).reshape(n, rec),
-                    ne=ne.cpu().numpy().astype(np.int64), nl=nl.cpu().numpy().astype(np.int64),
-                    rgb=rgb.cpu().numpy().reshape(n, 3), res=r)
-
-    def render(self, p, accum=None, accel=None, stream=None):
-        import torch
-
-        accel = accel or (self.conf if p.flags else self.fast)
-        if accum is None:
-            accum = torch.zeros(3 * p.width * p.height, dtype=torch.float32, device="cuda:0")
-        r = accel.RenderBDPT(p, accum.data_ptr(), stream)
-        return accum, r
-
-
-def slot_map(p):
-    """(pix, smp, valid) of every slot of a call: the path pass's tile map"""
-    from nanort_b200 import api
-
-    n = api.bdpt_slots(p)
-    tp = p.tile_w * p.tile_h
-    s = np.arange(n, dtype=np.int64)
-    k, rem = s // (tp * p.spp), s % (tp * p.spp)
-    smp, q = rem // tp, rem % tp
-    bw = p.tile_w // 8
-    blk, inn = q // 32, q % 32
-    lx, ly = (blk % bw) * 8 + (inn & 7), (blk // bw) * 4 + (inn >> 3)
-    tiles_x = -(-p.width // p.tile_w)
-    tile = k * p.n_shards + p.shard
-    x, y = (tile % tiles_x) * p.tile_w + lx, (tile // tiles_x) * p.tile_h + ly
-    valid = (x < p.width) & (y < p.height)
-    return y * p.width + x, smp, valid
-
-
-def frame_from_samples(p, ex, frame=None):
-    """d_accum as the device adds it: per pixel, the sample colours in ascending sample order"""
-    pix, smp, valid = slot_map(p)
-    frame = np.zeros((p.width * p.height, 3), np.float32) if frame is None else frame
-    for s in range(p.spp):
-        m = valid & (smp == s) & (ex["ne"] > 1)
-        frame[pix[m]] += ex["rgb"][m]
-    return frame
-
-
 @pytest.fixture(scope="module")
 def cornell(ref_mod):
     from nanort_b200 import scenes as S
 
     v, f, mats, ids, _ = S.cornell_with_materials()
     return Setup(ref_mod, v, f, mats, ids)
-
-
-def _bits(a):
-    return np.ascontiguousarray(a, np.float32).view(np.uint32)
 
 
 @pytest.mark.parametrize("flags", [1, 0], ids=["conformance", "production"])
@@ -147,44 +48,6 @@ def test_connections_bit_for_bit(cornell, flags):
             bad.append((int(i), want, ex["rgb"][i]))
     assert not bad, (len(bad), bad[:5])
     assert np.count_nonzero(ex["rgb"][live].sum(axis=1)) > 100  # the frame is not black
-
-
-FIELDS = ("position", "original_norm", "norm", "beta", "wo", "pdf_fwd", "pdf_rev")
-
-
-def _close(a, b, rel):
-    """|a - b| <= rel * the larger magnitude, per scalar or, for rows of vectors (position, normal, colour), per row:
-    a coordinate near 0 is held to the precision of its vector"""
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    scale = np.maximum(np.abs(a), np.abs(b))
-    if a.ndim > 1:
-        scale = scale.max(axis=-1, keepdims=True)
-    return bool(np.all(np.abs(a - b) <= rel * scale))
-
-
-def _compare_samples(setup, p, ex, slots):
-    """(structure matches, value mismatches) of the device's samples against bdpt_ref_sample"""
-    pix, smp, valid = slot_map(p)
-    same, diverged, value_bad = 0, [], []
-    for i in slots:
-        if not valid[i]:
-            continue
-        x, r = int(pix[i] % p.width), int(pix[i] // p.width)
-        y = p.height - 1 - r
-        seed = M.seed(x, y, p.width, p.spp_total, p.sample0 + int(smp[i]))
-        eye, light, rgb = setup.ref.sample(x, y, p.width, p.height, seed)
-        ge, gl = ex["eye"][i, :ex["ne"][i]], ex["light"][i, :ex["nl"][i]]
-        structure = len(eye) == len(ge) and len(light) == len(gl) and all(
-            np.array_equal(a[k], b[k]) for a, b in ((eye, ge), (light, gl)) for k in ("type", "prim_id", "material"))
-        if not structure:
-            diverged.append(int(i))
-            continue
-        same += 1
-        ok = all(_close(a[k], b[k], 1e-4) for a, b in ((eye, ge), (light, gl)) for k in FIELDS)
-        ok = ok and _close(rgb[None], ex["rgb"][i][None], 1e-3)
-        if not ok:
-            value_bad.append(int(i))
-    return same, diverged, value_bad
 
 
 def test_whole_samples_against_the_reference(cornell):
