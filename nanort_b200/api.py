@@ -69,6 +69,8 @@ BAKE_EXPORTS = ["nrt_uv_raster_device", "nrt_bake_ao_device", "nrt_bake_ao_rays_
 
 # every symbol include/nanort_b200_bdpt.h declares (the bidirectional path tracer)
 BDPT_EXPORTS = ["nrt_render_bdpt_device", "nrt_bdpt_export_device"]
+# every symbol include/nanort_b200_scene_bdpt.h declares (the bidirectional path tracer over scenes)
+SCENE_BDPT_EXPORTS = ["nrt_scene_render_bdpt_device", "nrt_scene_bdpt_export_device"]
 
 
 class NanortB200Error(RuntimeError):
@@ -249,6 +251,8 @@ def lib():
     L.nrt_bake_ao_rays_device.argtypes = [vp, vp, C.POINTER(BakeParams), vp, C.c_uint64, u64p, vp]
     L.nrt_render_bdpt_device.argtypes = [vp, C.POINTER(BdptParams), vp, C.POINTER(BdptResult), vp]
     L.nrt_bdpt_export_device.argtypes = [vp, C.POINTER(BdptParams), vp, vp, vp, vp, vp, C.POINTER(BdptResult), vp]
+    L.nrt_scene_render_bdpt_device.argtypes = [vp, C.POINTER(BdptParams), vp, vp, C.POINTER(BdptResult), vp]
+    L.nrt_scene_bdpt_export_device.argtypes = [vp, C.POINTER(BdptParams), vp] + [vp] * 8 + [C.POINTER(BdptResult), vp]
     L.nrt_build_f64.argtypes = [vp, sz, sz, vp, u32, vp, C.POINTER(vp)]
     L.nrt_build_f64_ex.argtypes = [vp, sz, sz, vp, u32, vp, u32, C.POINTER(vp)]
     L.nrt_adopt_f64.argtypes = [vp, sz, vp, sz, vp, sz, sz, vp, u32, C.POINTER(vp)]
@@ -787,6 +791,29 @@ class Scene:
                                                   vp(d_accum_rgb), C.byref(nc), C.byref(ns), 1 if skip_shadow_pass else 0,
                                                   vp(stream) if stream else None))
         return int(nc.value), int(ns.value)
+
+    def RenderBDPT(self, params: "BdptParams", shading, d_accum_rgb_ptr, stream=None, want_result=True):
+        """The bidirectional path tracer over the two-level scene (nrt_scene_render_bdpt_device): BVHAccel.RenderBDPT's
+        parameters without material ids or normals, which come per instance in `shading` (a list of SceneShading,
+        both pointers required)."""
+        res = BdptResult()
+        _check(lib().nrt_scene_render_bdpt_device(self._h, C.byref(params), C.cast(self._shading(shading), C.c_void_p),
+                                                  C.c_void_p(d_accum_rgb_ptr), C.byref(res) if want_result else None,
+                                                  C.c_void_p(stream) if stream else None))
+        return res if want_result else None
+
+    def ExportBDPT(self, params: "BdptParams", shading, d_eye_ptr, d_light_ptr, d_eye_inst_ptr, d_light_inst_ptr,
+                   d_light_pair_ptr, d_n_eye_ptr, d_n_light_ptr, d_sample_rgb_ptr, stream=None):
+        """RenderBDPT's samples per slot (nrt_scene_bdpt_export_device): BVHAccel.ExportBDPT's buffers, plus the
+        instance of every vertex record (uint32) and each slot's sampled light {instance, face} (uint32[2])."""
+        res = BdptResult()
+        vp = C.c_void_p
+        _check(lib().nrt_scene_bdpt_export_device(self._h, C.byref(params), C.cast(self._shading(shading), vp),
+                                                  vp(d_eye_ptr), vp(d_light_ptr), vp(d_eye_inst_ptr),
+                                                  vp(d_light_inst_ptr), vp(d_light_pair_ptr), vp(d_n_eye_ptr),
+                                                  vp(d_n_light_ptr), vp(d_sample_rgb_ptr), C.byref(res),
+                                                  vp(stream) if stream else None))
+        return res
 
 
 # ------------------------------------------------------------------ BVHAccel<double>
