@@ -71,6 +71,8 @@ BAKE_EXPORTS = ["nrt_uv_raster_device", "nrt_bake_ao_device", "nrt_bake_ao_rays_
 BDPT_EXPORTS = ["nrt_render_bdpt_device", "nrt_bdpt_export_device"]
 # every symbol include/nanort_b200_scene_bdpt.h declares (the bidirectional path tracer over scenes)
 SCENE_BDPT_EXPORTS = ["nrt_scene_render_bdpt_device", "nrt_scene_bdpt_export_device"]
+# every symbol include/nanort_b200_lightmap.h declares (path-traced lightmaps of UV atlases)
+LIGHTMAP_EXPORTS = ["nrt_bake_lightmap_device", "nrt_bake_lightmap_bounce_device"]
 
 
 class NanortB200Error(RuntimeError):
@@ -152,6 +154,29 @@ class BakeParams(C.Structure):
 class BakeResult(C.Structure):
     _fields_ = [
         ("texels", C.c_uint64), ("ao_rays", C.c_uint64), ("ao_hits", C.c_uint64),
+        ("traverse_ms", C.c_float), ("total_ms", C.c_float),
+        ("launches", C.c_uint32), ("traverse_launches", C.c_uint32),
+    ]
+
+
+class LightmapParams(C.Structure):
+    """nrt_lightmap_params: the records' atlas, samples sample0 .. sample0+spp-1, max_bounces, the continuation rays'
+    range, the path pass's materials, material ids, emissive faces and face-varying normals (device pointers),
+    TRAVERSE_ANY_HIT / TRAVERSE_CPP03_INVERSE flags."""
+    _fields_ = [
+        ("width", C.c_uint32), ("height", C.c_uint32),
+        ("spp", C.c_uint32), ("sample0", C.c_uint32), ("seed", C.c_uint32), ("max_bounces", C.c_uint32),
+        ("ray_min_t", C.c_float), ("ray_max_t", C.c_float),
+        ("n_materials", C.c_uint32), ("n_emissive", C.c_uint32),
+        ("d_materials", C.c_void_p), ("d_material_ids", C.c_void_p), ("d_emissive_faces", C.c_void_p),
+        ("d_facevarying_normals", C.c_void_p),
+        ("flags", C.c_uint32), ("pad", C.c_uint32),
+    ]
+
+
+class LightmapResult(C.Structure):
+    _fields_ = [
+        ("texels", C.c_uint64), ("paths", C.c_uint64), ("radiance_rays", C.c_uint64), ("shadow_rays", C.c_uint64),
         ("traverse_ms", C.c_float), ("total_ms", C.c_float),
         ("launches", C.c_uint32), ("traverse_launches", C.c_uint32),
     ]
@@ -249,6 +274,9 @@ def lib():
     L.nrt_uv_raster_device.argtypes = [vp, vp, C.POINTER(UvRasterParams), vp, vp, vp, vp, u64p, vp]
     L.nrt_bake_ao_device.argtypes = [vp, vp, C.POINTER(BakeParams), vp, C.POINTER(BakeResult), vp]
     L.nrt_bake_ao_rays_device.argtypes = [vp, vp, C.POINTER(BakeParams), vp, C.c_uint64, u64p, vp]
+    L.nrt_bake_lightmap_device.argtypes = [vp, vp, C.POINTER(LightmapParams), vp, C.POINTER(LightmapResult), vp]
+    L.nrt_bake_lightmap_bounce_device.argtypes = [vp, vp, C.POINTER(LightmapParams), u32, C.c_uint64] + [vp] * 11 + [
+        u64p, u64p, C.c_int, vp]
     L.nrt_render_bdpt_device.argtypes = [vp, C.POINTER(BdptParams), vp, C.POINTER(BdptResult), vp]
     L.nrt_bdpt_export_device.argtypes = [vp, C.POINTER(BdptParams), vp, vp, vp, vp, vp, C.POINTER(BdptResult), vp]
     L.nrt_scene_render_bdpt_device.argtypes = [vp, C.POINTER(BdptParams), vp, vp, C.POINTER(BdptResult), vp]
@@ -646,6 +674,33 @@ class BVHAccel:
         _check(lib().nrt_bake_ao_rays_device(self._h, C.c_void_p(d_records_ptr), C.byref(params), C.c_void_p(d_rays_ptr),
                                              int(capacity), C.byref(n), C.c_void_p(stream) if stream else None))
         return int(n.value)
+
+    def BakeLightmap(self, d_records_ptr, params: LightmapParams, d_accum_rgb_ptr, stream=None, want_result=True):
+        """Path-traced lightmap from every covered texel of UVRaster's records, traced against this (world) accel
+        (nrt_bake_lightmap_device): d_accum_rgb[3 * texel + c] (float[3 * width * height]) gains the texel's path
+        estimates; divided by spp it estimates irradiance / pi, and times a diffuse albedo the outgoing diffuse radiance.
+        Ordered on the device with the accel's other passes, like RenderPath."""
+        res = LightmapResult()
+        _check(lib().nrt_bake_lightmap_device(self._h, C.c_void_p(d_records_ptr), C.byref(params),
+                                              C.c_void_p(d_accum_rgb_ptr), C.byref(res) if want_result else None,
+                                              C.c_void_p(stream) if stream else None))
+        return res if want_result else None
+
+    def LightmapBounce(self, d_records_ptr, params: LightmapParams, bounce, n_rays, d_org_tmin, d_dir_tmax, d_path_id,
+                       d_weight, d_out_org_tmin, d_out_dir_tmax, d_out_path_id, d_sh_org_tmin, d_sh_dir_tmax,
+                       d_sh_contrib_pix, d_accum_rgb, skip_shadow_pass=False, stream=None):
+        """nrt_bake_lightmap_bounce_device: one bounce of BakeLightmap on caller-owned device queues, path id = slot of
+        the call (bounce 0: the texel vertex of paths [0, n_rays), the input queue is ignored); returns
+        (n_continue, n_shadow)."""
+        nc, ns = C.c_uint64(0), C.c_uint64(0)
+        vp = C.c_void_p
+        opt = lambda x: vp(x) if x else None
+        _check(lib().nrt_bake_lightmap_bounce_device(
+            self._h, vp(d_records_ptr), C.byref(params), int(bounce), int(n_rays), opt(d_org_tmin), opt(d_dir_tmax),
+            opt(d_path_id), vp(d_weight), vp(d_out_org_tmin), vp(d_out_dir_tmax), vp(d_out_path_id), vp(d_sh_org_tmin),
+            vp(d_sh_dir_tmax), vp(d_sh_contrib_pix), vp(d_accum_rgb), C.byref(nc), C.byref(ns),
+            1 if skip_shadow_pass else 0, vp(stream) if stream else None))
+        return int(nc.value), int(ns.value)
 
     def RenderBDPT(self, params: BdptParams, d_accum_rgb_ptr, stream=None, want_result=True):
         """The reference's bidirectional path tracer (nrt_render_bdpt_device): each sample's connectPath colour is

@@ -73,14 +73,41 @@ uint32_t scan_launches(uint32_t n) {
   return n == 0 ? 0u : tiles > 1 ? 2u + scan_launches(tiles) : 1u;
 }
 
-// texel indices are uint32, and the scan indexes its tiles in uint32
-constexpr uint64_t kMaxTexels = 1ull << 31;
+}  // namespace
 
 bool is_triangle_accel(const Accel *a) {
   return a->prim_kind == 0 && !a->d_prim_boxes && a->d_faces && a->d_verts && a->d_pair && a->d_tris_cm;
 }
 
-}  // namespace
+// Compacts the covered texels of the n records into `list` and reads their count back, under the world accel's pass
+// ordering, which the caller holds; d_wave holds at least (2 n + scan_scratch_words(n)) words.  Refuses (after the
+// compaction's launches, before any traversal) records whose prim_id is neither a miss nor a face of `a`.  The AO
+// bake and the lightmap bake (lightmap.cu) start here.
+int bake_prepare(Accel *a, const void *d_records, uint32_t n, const char *who, cudaStream_t s, uint32_t **list,
+                 uint32_t *n_cov, uint32_t *launches) {
+  uint32_t *offs = static_cast<uint32_t *>(a->d_wave);
+  *list = offs + n;
+  uint32_t *scratch = *list + n;
+  unsigned long long *info = reinterpret_cast<unsigned long long *>(a->d_counters) + 2;  // [2] covered, [3] bad record
+  const Hit16 *rec = static_cast<const Hit16 *>(d_records);
+  NRT_CUDA(cudaMemsetAsync(info, 0, 2 * sizeof(unsigned long long), s));
+  covered_flags_kernel<<<(n + 255) / 256, 256, 0, s>>>(rec, n, a->n_prims, offs, info);
+  NRT_CUDA(cudaGetLastError());
+  if (const int rc = exclusive_scan_u32_async(offs, offs, n, scratch, s)) return rc;
+  compact_texels_kernel<<<(n + 255) / 256, 256, 0, s>>>(rec, n, offs, *list, info);
+  NRT_CUDA(cudaGetLastError());
+  *launches += 2 + scan_launches(n);
+  unsigned long long h[2] = {0, 0};
+  NRT_CUDA(cudaMemcpyAsync(h, info, sizeof(h), cudaMemcpyDeviceToHost, s));
+  NRT_CUDA(cudaStreamSynchronize(s));
+  if (h[1]) {
+    set_error(std::string(who) + ": a record's prim_id is not a face of the world accel");
+    return NRT_ERR_INVALID;
+  }
+  *n_cov = (uint32_t)h[0];
+  return NRT_OK;
+}
+
 }  // namespace nrt
 
 using namespace nrt;
@@ -169,34 +196,6 @@ extern "C" int nrt_uv_raster_device(const nrt_accel *uv_h, const nrt_accel *worl
   return NRT_OK;
 }
 
-// Checks the arguments of a bake, then (under the world accel's pass ordering, which the caller holds) compacts the
-// covered texels into `list` and reads their count back.  Launches nothing when it refuses.
-static int bake_prepare(Accel *a, const void *d_records, const nrt_bake_params &p, const char *who, cudaStream_t s,
-                        uint32_t **list, uint32_t *n_cov, uint32_t *launches) {
-  uint32_t *offs = static_cast<uint32_t *>(a->d_wave);
-  const uint32_t n = p.width * p.height;
-  *list = offs + n;
-  uint32_t *scratch = *list + n;
-  unsigned long long *info = reinterpret_cast<unsigned long long *>(a->d_counters) + 2;  // [2] covered, [3] bad record
-  const Hit16 *rec = static_cast<const Hit16 *>(d_records);
-  NRT_CUDA(cudaMemsetAsync(info, 0, 2 * sizeof(unsigned long long), s));
-  covered_flags_kernel<<<(n + 255) / 256, 256, 0, s>>>(rec, n, a->n_prims, offs, info);
-  NRT_CUDA(cudaGetLastError());
-  if (const int rc = exclusive_scan_u32_async(offs, offs, n, scratch, s)) return rc;
-  compact_texels_kernel<<<(n + 255) / 256, 256, 0, s>>>(rec, n, offs, *list, info);
-  NRT_CUDA(cudaGetLastError());
-  *launches += 2 + scan_launches(n);
-  unsigned long long h[2] = {0, 0};
-  NRT_CUDA(cudaMemcpyAsync(h, info, sizeof(h), cudaMemcpyDeviceToHost, s));
-  NRT_CUDA(cudaStreamSynchronize(s));
-  if (h[1]) {
-    set_error(std::string(who) + ": a record's prim_id is not a face of the world accel");
-    return NRT_ERR_INVALID;
-  }
-  *n_cov = (uint32_t)h[0];
-  return NRT_OK;
-}
-
 static int bake_check(const Accel *a, const void *d_records, const nrt_bake_params *p, const char *who) {
   if (!a || !d_records || !p) {
     set_error(std::string(who) + ": NULL argument");
@@ -279,7 +278,7 @@ static int run_bake(const nrt_accel *h, const void *d_records, const nrt_bake_pa
     NRT_CUDA(cudaEventRecord(e_begin, s));
   }
   uint32_t *list = nullptr, n_cov = 0;
-  if (const int rc = bake_prepare(a, d_records, p, who, s, &list, &n_cov, &launches)) return rc;
+  if (const int rc = bake_prepare(a, d_records, n, who, s, &list, &n_cov, &launches)) return rc;
   const uint64_t total = (uint64_t)n_cov * p.spp;
   if (n_rays) *n_rays = total;
   if (dump && total > capacity) {

@@ -166,7 +166,7 @@ extern "C" int nrt_render_path_device(const nrt_accel *h, const nrt_path_params 
         ev.push_back(t1);
         cudaEventRecord(t0, s);
       }
-      PathShadeEpilogue epi{p, s0, in, b, q, a->d_verts, a->d_faces, d_accum_rgb, ctr};
+      PathShadeEpilogue epi{p, TileSlots{s0}, in, b, q, a->d_verts, a->d_faces, d_accum_rgb, ctr};
       rc = launch_traverse_path_radiance(a, epi, ctr + 3, count, opt, trav_flags, s);
       if (rc != NRT_OK) break;
       rc = launch_traverse_path_shadow(a, q, ctr + 1, count, d_accum_rgb, opt, trav_flags, s);
@@ -259,7 +259,7 @@ extern "C" int nrt_path_bounce_device(const nrt_accel *h, const nrt_path_params 
   NRT_CUDA(cudaMemcpyAsync(ctr, init, sizeof(init), cudaMemcpyHostToDevice, s));
   const TraceOptions16 opt = default_trace_options();
   const uint32_t trav_flags = p.flags & 0xFFFFu;
-  PathShadeEpilogue epi{p, 0ull, 0, bounce, q, a->d_verts, a->d_faces, d_accum_rgb, ctr};
+  PathShadeEpilogue epi{p, TileSlots{0ull}, 0, bounce, q, a->d_verts, a->d_faces, d_accum_rgb, ctr};
   int rc = launch_traverse_path_radiance(a, epi, ctr + 3, (size_t)n_rays, opt, trav_flags, s);
   if (rc != NRT_OK) return rc;
   if (!skip_shadow_pass) {

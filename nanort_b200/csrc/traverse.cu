@@ -378,6 +378,13 @@ int launch_traverse_path_radiance(const Accel *a, const PathShadeEpilogue &epi, 
       a, SoaRays{epi.q.org_tmin[epi.in], epi.q.dir_tmax[epi.in]}, capacity, d_count, epi, opt, flags, s);
 }
 
+// the lightmap bake's bounces 1 and up (lightmap.cu): the path radiance launch with the texel slot map
+int launch_traverse_lightmap_radiance(const Accel *a, const LightmapShadeEpilogue &epi, const unsigned long long *d_count,
+                                      size_t capacity, const TraceOptions16 &opt, uint32_t flags, cudaStream_t s) {
+  return launch_fused<LightmapShadeEpilogue, PathRadiancePolicy>(
+      a, SoaRays{epi.q.org_tmin[epi.in], epi.q.dir_tmax[epi.in]}, capacity, d_count, epi, opt, flags, s);
+}
+
 int launch_traverse_path_shadow(const Accel *a, const PathQueues &q, const unsigned long long *d_count,
                                 size_t capacity, float *d_accum, const TraceOptions16 &opt, uint32_t flags,
                                 cudaStream_t s) {

@@ -376,6 +376,9 @@ struct AoAccumulateEpilogue {
 };
 
 // ------------------------------------------------------------------ texture-space baking (bake.cu)
+// texel indices are uint32, and the scan indexes its tiles in uint32
+constexpr uint64_t kMaxTexels = 1ull << 31;
+
 // Texel cast of the reference's uv_raster (examples/uv_raster/main.cc:752-770): ray i is texel (i % width, i / width),
 // generated at fetch.  Payload: the texel its record goes to, after the flips (main.cc:779-782).
 struct TexelRays {
@@ -464,6 +467,35 @@ struct TexelStoreEpilogue {
   }
 };
 
+// The surface point of a covered texel: P = the position AOV (lerp3 of the record's world triangle) and the bake's
+// normal, the unit geometric normal as wound (Accel::d_face_n), flipped to the side of the interpolated face-varying
+// normal when those are given.  The AO bake's rays and the lightmap's texel vertex start here.
+__device__ __forceinline__ void texel_point(const float4 *__restrict__ records, const float *__restrict__ verts,
+                                            const uint32_t *__restrict__ faces, const float4 *__restrict__ face_n,
+                                            const float *__restrict__ fv_normals, uint32_t texel, float &ox, float &oy,
+                                            float &oz, float &nx, float &ny, float &nz) {
+  const float4 r = __ldg(records + texel);
+  const float u = r.x, v = r.y;
+  const uint32_t prim = __float_as_uint(r.w);
+  const uint32_t *f = faces + 3 * (size_t)prim;
+  lerp3(verts + 3 * (size_t)__ldg(f), verts + 3 * (size_t)__ldg(f + 1), verts + 3 * (size_t)__ldg(f + 2), u, v, ox, oy,
+        oz);
+  const float4 n = __ldg(face_n + prim);
+  nx = n.x;
+  ny = n.y;
+  nz = n.z;
+  if (fv_normals) {  // the geometric normal, on the side of the interpolated shading normal
+    const float *fn = fv_normals + 9 * (size_t)prim;
+    float sx, sy, sz;
+    lerp3(fn, fn + 3, fn + 6, u, v, sx, sy, sz);
+    if (nx * sx + ny * sy + nz * sz < 0.0f) {
+      nx = -nx;
+      ny = -ny;
+      nz = -nz;
+    }
+  }
+}
+
 // AO rays of the bake: slot i of a launch is sample sample0 + i / n_cov of covered texel texels[i % n_cov], with the
 // texel's record (nrt_uv_raster_device) giving the world triangle and the barycentrics.  Payload: the texel.
 struct BakeAoRays {
@@ -483,24 +515,8 @@ struct BakeAoRays {
     uint32_t s, k;
     n_cov.divmod((uint32_t)i, s, k);
     const uint32_t texel = __ldg(texels + k), smp = sample0 + s;
-    const float4 r = __ldg(records + texel);
-    const float u = r.x, v = r.y;
-    const uint32_t prim = __float_as_uint(r.w);
-    const uint32_t *f = faces + 3 * (size_t)prim;
-    lerp3(verts + 3 * (size_t)__ldg(f), verts + 3 * (size_t)__ldg(f + 1), verts + 3 * (size_t)__ldg(f + 2), u, v, ox,
-          oy, oz);
-    const float4 n = __ldg(face_n + prim);
-    float nx = n.x, ny = n.y, nz = n.z;
-    if (fv_normals) {  // the geometric normal, on the side of the interpolated shading normal
-      const float *fn = fv_normals + 9 * (size_t)prim;
-      float sx, sy, sz;
-      lerp3(fn, fn + 3, fn + 6, u, v, sx, sy, sz);
-      if (nx * sx + ny * sy + nz * sz < 0.0f) {
-        nx = -nx;
-        ny = -ny;
-        nz = -nz;
-      }
-    }
+    float nx, ny, nz;
+    texel_point(records, verts, faces, face_n, fv_normals, texel, ox, oy, oz, nx, ny, nz);
     ao_direction(nx, ny, nz, texel, smp, seed, dx, dy, dz);
     tmin = min_t;
     tmax = max_t;
@@ -592,7 +608,9 @@ struct FlatSpawn {
 // roulette.  (nx, ny, nz) is originalNorm; w the path's throughput + do_emission, written back to *wslot when the path
 // continues.  Lights (FlatLights, or the scene pass's world-space records) give the light sample; Spawn places the
 // continuation and shadow rays.  Returns in cont / shadow whether this lane appends a continuation or a shadow ray.
-template <class Lights, class Spawn>
+// ONE_SIDED: a light sample below the (flipped) normal, dot(l, n) <= 0, contributes nothing and spawns no shadow ray,
+// instead of the reference's |cos| -- the lightmap's texel vertex, a receiver that only sees its own hemisphere.
+template <class Lights, class Spawn, bool ONE_SIDED = false>
 __device__ __forceinline__ void path_shade_hit(const nrt_path_params &p, uint32_t bounce, uint32_t pix, uint32_t smp,
                                                float4 o, float4 d, float t, float nx, float ny, float nz,
                                                const PathMaterial *mat, const Lights &lights, const Spawn &spawn,
@@ -661,8 +679,9 @@ __device__ __forceinline__ void path_shade_hit(const nrt_path_params &p, uint32_
         // 943-950): those Traverse calls are part of its loop, so they are part of ours.
         const float cos_l = fmaxf(-(lx * lnx + ly * lny + lz * lnz), 0.0f);
         const float pdf = (1.0f / nf) * (1.0f / area) * (dist * dist) / fabsf(cos_l);  // PdfAtoW
-        if (pdf > 0.0f) {
-          const float cos_t = fabsf(lx * nx + ly * ny + lz * nz);
+        const float cos_s = lx * nx + ly * ny + lz * nz;
+        if (pdf > 0.0f && (!ONE_SIDED || cos_s > 0.0f)) {
+          const float cos_t = fabsf(cos_s);
           const float k = (1.0f / 3.14159265358979f) * cos_l * cos_t / pdf;  // brdf * cosine EDF * cos / pdf
           spawn.shadow(p, Px, Py, Pz, lx, ly, lz, dist, lnx, lny, lnz, so, sd);
           sc = make_float4(k * m.diffuse[0] * lex * w.x, k * m.diffuse[1] * ley * w.y, k * m.diffuse[2] * lez * w.z,
@@ -761,12 +780,42 @@ __device__ __forceinline__ void path_append(const PathQueues &q, int out, unsign
   }
 }
 
+// Slot maps of the radiance retire step: path id -> (pixel or texel, sample), the pair that keys rand_ps and picks the
+// accumulation index.  False: the slot carries no path.
+// The path pass: slot slot0 + pid of the tile map (slot_to_pixel), samples counted from p.sample0.
+struct TileSlots {
+  unsigned long long slot0;
+  __device__ __forceinline__ bool operator()(const nrt_path_params &p, uint32_t pid, uint32_t &pix, uint32_t &smp) const {
+    if (!slot_to_pixel(tile_map(p), slot0 + pid, pix, smp)) return false;
+    smp += p.sample0;
+    return true;
+  }
+};
+
+// The lightmap bake: slot s = base + pid of a call is sample p.sample0 + s / n_cov of covered texel texels[s % n_cov].
+// The 64-bit wave base enters as base / n_cov (base_sample) and base % n_cov (base_k), so that base_k + pid, below
+// 2^31 + 2^23 in a wave and a 32-bit path id at base 0, takes the 32-bit FastDiv.
+struct TexelSlots {
+  const uint32_t *texels;  // covered texels, ascending
+  FastDiv n_cov;
+  uint32_t base_k, base_sample;
+  __device__ __forceinline__ bool operator()(const nrt_path_params &p, uint32_t pid, uint32_t &texel,
+                                             uint32_t &smp) const {
+    uint32_t s, k;
+    n_cov.divmod(base_k + pid, s, k);
+    texel = __ldg(texels + k);
+    smp = p.sample0 + base_sample + s;
+    return true;
+  }
+};
+
 // Radiance rays of bounce `bounce`: the retire step is the reference's per-hit shading block
 // (examples/path_tracer/main.cc:856-976): normal, then path_shade_hit.
-struct PathShadeEpilogue {
+template <class Slots>
+struct PathShadeEpilogueT {
   static constexpr bool kAnyHit = false;
   nrt_path_params p;
-  unsigned long long slot0;
+  Slots slots;
   int in;  // which radiance queue is being traversed; (in ^ 1) receives the continuation rays
   uint32_t bounce;
   PathQueues q;
@@ -782,8 +831,7 @@ struct PathShadeEpilogue {
     if (retiring && t < max_t) {
       pid = q.path_id[in][ray_idx];
       uint32_t pix, smp;
-      if (slot_to_pixel(tile_map(p), slot0 + pid, pix, smp)) {
-        smp += p.sample0;
+      if (slots(p, pid, pix, smp)) {
         const float4 o = q.org_tmin[in][ray_idx], d = q.dir_tmax[in][ray_idx];
         const float4 w = q.weight[pid];  // throughput rgb, w.w = do_emission (no light sampling at the previous event)
         const PathMaterial *mats = reinterpret_cast<const PathMaterial *>(p.d_materials);
@@ -821,6 +869,35 @@ struct PathShadeEpilogue {
     path_append(q, in ^ 1, counters, cont, shadow, pid, co, cd, so, sd, sc);
   }
 };
+typedef PathShadeEpilogueT<TileSlots> PathShadeEpilogue;    // the path pass (path.cu)
+typedef PathShadeEpilogueT<TexelSlots> LightmapShadeEpilogue;  // the lightmap bake's bounces 1 and up (lightmap.cu)
+
+// Bounce 0 of the lightmap bake for path `pid`: no ray is traced.  The texel's surface point (texel_point) is shaded
+// by path_shade_hit as a white Lambertian seen along its normal -- a ray (P, -n) that hit at t = 0, whose lobe choice
+// is then always the diffuse one with albedo (1, 1, 1): next-event estimation from random dimensions 8 and 9, a cosine
+// continuation from 10 and 11 with weight 1 and do_emission 0.  ONE_SIDED: a light sample below the texel's
+// hemisphere contributes nothing and spawns no shadow ray.  Returns the appends as path_shade_hit does.
+__device__ __forceinline__ void lightmap_texel_vertex(const nrt_path_params &p, const TexelSlots &slots, uint32_t pid,
+                                                      const float4 *records, const float *verts, const uint32_t *faces,
+                                                      const float4 *face_n, float4 *wslot, float *accum, bool &cont,
+                                                      bool &shadow, float4 &co, float4 &cd, float4 &so, float4 &sd,
+                                                      float4 &sc) {
+  uint32_t texel, smp;
+  slots(p, pid, texel, smp);
+  float Px, Py, Pz, nx, ny, nz;
+  texel_point(records, verts, faces, face_n, reinterpret_cast<const float *>(p.d_facevarying_normals), texel, Px, Py,
+              Pz, nx, ny, nz);
+  PathMaterial white = {};
+  white.diffuse[0] = white.diffuse[1] = white.diffuse[2] = 1.0f;
+  white.ior = 1.0f;
+  const PathMaterial *mats = reinterpret_cast<const PathMaterial *>(p.d_materials);
+  const uint32_t *mat_ids = reinterpret_cast<const uint32_t *>(p.d_material_ids);
+  const uint32_t *emissive = reinterpret_cast<const uint32_t *>(p.d_emissive_faces);
+  path_shade_hit<FlatLights, FlatSpawn, true>(
+      p, 0u, texel, smp, make_float4(Px, Py, Pz, p.ray_min_t), make_float4(-nx, -ny, -nz, p.ray_max_t), 0.0f, nx, ny,
+      nz, &white, FlatLights{verts, faces, emissive, mat_ids, mats}, FlatSpawn{}, make_float4(1.0f, 1.0f, 1.0f, 1.0f),
+      wslot, accum, cont, shadow, co, cd, so, sd, sc);
+}
 
 // Shadow rays: an unoccluded light sample adds its contribution (CheckForOccluder returned false)
 struct ShadowAccumulateEpilogue {
