@@ -73,6 +73,9 @@ BDPT_EXPORTS = ["nrt_render_bdpt_device", "nrt_bdpt_export_device"]
 SCENE_BDPT_EXPORTS = ["nrt_scene_render_bdpt_device", "nrt_scene_bdpt_export_device"]
 # every symbol include/nanort_b200_lightmap.h declares (path-traced lightmaps of UV atlases)
 LIGHTMAP_EXPORTS = ["nrt_bake_lightmap_device", "nrt_bake_lightmap_bounce_device"]
+# every symbol include/nanort_b200_scene_bake.h declares (texel cast, AO and lightmap bakes of two-level scenes)
+SCENE_BAKE_EXPORTS = ["nrt_scene_uv_raster_device", "nrt_scene_bake_ao_device", "nrt_scene_bake_ao_rays_device",
+                      "nrt_scene_bake_lightmap_device", "nrt_scene_bake_lightmap_bounce_device"]
 
 
 class NanortB200Error(RuntimeError):
@@ -182,6 +185,17 @@ class LightmapResult(C.Structure):
     ]
 
 
+class SceneChart(C.Structure):
+    """nrt_scene_chart: one instance's rectangle of the atlas (x0, y0, width, height) and the texel cast that fills it:
+    the instance's UV accel (a BVHAccel handle, None for no chart), uv_region, texel_offset, flips."""
+    _fields_ = [
+        ("uv", C.c_void_p),
+        ("x0", C.c_uint32), ("y0", C.c_uint32), ("width", C.c_uint32), ("height", C.c_uint32),
+        ("uv_region", C.c_float * 4), ("texel_offset", C.c_float * 2),
+        ("flip_x", C.c_uint32), ("flip_y", C.c_uint32),
+    ]
+
+
 class BdptParams(C.Structure):
     """nrt_bdpt_params: camera {org, right, up, forward}, image, samples sample0 .. sample0+spp-1 of spp_total, the path
     pass's tile map, max_bounces, materials (16 floats each), material ids and face-varying normals (device pointers),
@@ -277,6 +291,13 @@ def lib():
     L.nrt_bake_lightmap_device.argtypes = [vp, vp, C.POINTER(LightmapParams), vp, C.POINTER(LightmapResult), vp]
     L.nrt_bake_lightmap_bounce_device.argtypes = [vp, vp, C.POINTER(LightmapParams), u32, C.c_uint64] + [vp] * 11 + [
         u64p, u64p, C.c_int, vp]
+    L.nrt_scene_uv_raster_device.argtypes = [vp, vp, u32, u32, u32, vp, vp, vp, vp, vp, u64p, vp]
+    L.nrt_scene_bake_ao_device.argtypes = [vp, vp, vp, vp, C.POINTER(BakeParams), vp, C.POINTER(BakeResult), vp]
+    L.nrt_scene_bake_ao_rays_device.argtypes = [vp, vp, vp, vp, C.POINTER(BakeParams), vp, C.c_uint64, u64p, vp]
+    L.nrt_scene_bake_lightmap_device.argtypes = [vp, vp, vp, C.POINTER(LightmapParams), vp, vp,
+                                                 C.POINTER(LightmapResult), vp]
+    L.nrt_scene_bake_lightmap_bounce_device.argtypes = [vp, vp, vp, C.POINTER(LightmapParams), vp, u32,
+                                                        C.c_uint64] + [vp] * 11 + [u64p, u64p, C.c_int, vp]
     L.nrt_render_bdpt_device.argtypes = [vp, C.POINTER(BdptParams), vp, C.POINTER(BdptResult), vp]
     L.nrt_bdpt_export_device.argtypes = [vp, C.POINTER(BdptParams), vp, vp, vp, vp, vp, C.POINTER(BdptResult), vp]
     L.nrt_scene_render_bdpt_device.argtypes = [vp, C.POINTER(BdptParams), vp, vp, C.POINTER(BdptResult), vp]
@@ -869,6 +890,83 @@ class Scene:
                                                   vp(d_n_light_ptr), vp(d_sample_rgb_ptr), C.byref(res),
                                                   vp(stream) if stream else None))
         return res
+
+    # -- texture-space baking over the scene (include/nanort_b200_scene_bake.h)
+    def _charts(self, charts):
+        assert len(charts) == len(self._nodes), "one SceneChart per instance"
+        arr = (SceneChart * len(charts))()
+        for i, c in enumerate(charts):
+            arr[i] = c
+        return arr
+
+    def UVRaster(self, charts, atlas_width, atlas_height, d_records_ptr, d_instance_ptr, shading=None,
+                 d_position_ptr=None, d_normal_ptr=None, flags=TRAVERSE_FAST, stream=None):
+        """The texel cast of an atlas with one chart per instance (nrt_scene_uv_raster_device): charts is a list of
+        SceneChart, one per instance; writes the hit records (HIT_DTYPE), the owning instance (uint32) and optionally
+        the world-space position / normal AOVs (float3) of every atlas texel.  Normals need `shading` (a list of
+        SceneShading with face-varying normals).  Returns the number of covered texels (synchronises `stream`)."""
+        n = C.c_uint64(0)
+        vp = C.c_void_p
+        opt = lambda x: vp(x) if x else None
+        sh = C.cast(self._shading(shading), vp) if shading is not None else None
+        _check(lib().nrt_scene_uv_raster_device(self._h, C.cast(self._charts(charts), vp), int(atlas_width),
+                                                int(atlas_height), int(flags), sh, vp(d_records_ptr),
+                                                vp(d_instance_ptr), opt(d_position_ptr), opt(d_normal_ptr), C.byref(n),
+                                                vp(stream) if stream else None))
+        return int(n.value)
+
+    def BakeAO(self, d_records_ptr, d_instance_ptr, params: "BakeParams", d_accum_ptr, shading=None, stream=None,
+               want_result=True):
+        """Cosine AO from every covered texel of UVRaster's records over the scene (nrt_scene_bake_ao_device):
+        d_accum[texel] += 1 per unoccluded ray; face-varying normals per instance through `shading` (or None)."""
+        res = BakeResult()
+        vp = C.c_void_p
+        sh = C.cast(self._shading(shading), vp) if shading is not None else None
+        _check(lib().nrt_scene_bake_ao_device(self._h, vp(d_records_ptr), vp(d_instance_ptr), sh, C.byref(params),
+                                              vp(d_accum_ptr), C.byref(res) if want_result else None,
+                                              vp(stream) if stream else None))
+        return res if want_result else None
+
+    def ExportBakeRays(self, d_records_ptr, d_instance_ptr, params: "BakeParams", d_rays_ptr, capacity, shading=None,
+                       stream=None):
+        """BakeAO's rays as 36-byte records in slot order (nrt_scene_bake_ao_rays_device); returns their count."""
+        n = C.c_uint64(0)
+        vp = C.c_void_p
+        sh = C.cast(self._shading(shading), vp) if shading is not None else None
+        _check(lib().nrt_scene_bake_ao_rays_device(self._h, vp(d_records_ptr), vp(d_instance_ptr), sh, C.byref(params),
+                                                   vp(d_rays_ptr), int(capacity), C.byref(n),
+                                                   vp(stream) if stream else None))
+        return int(n.value)
+
+    def BakeLightmap(self, d_records_ptr, d_instance_ptr, params: "LightmapParams", shading, d_accum_rgb_ptr,
+                     stream=None, want_result=True):
+        """Path-traced lightmap from every covered texel of UVRaster's records over the scene
+        (nrt_scene_bake_lightmap_device): BVHAccel.BakeLightmap's estimate with RenderPath's per-instance `shading`
+        and {instance, face} emissive pairs."""
+        res = LightmapResult()
+        vp = C.c_void_p
+        _check(lib().nrt_scene_bake_lightmap_device(self._h, vp(d_records_ptr), vp(d_instance_ptr), C.byref(params),
+                                                    C.cast(self._shading(shading), vp), vp(d_accum_rgb_ptr),
+                                                    C.byref(res) if want_result else None,
+                                                    vp(stream) if stream else None))
+        return res if want_result else None
+
+    def LightmapBounce(self, d_records_ptr, d_instance_ptr, params: "LightmapParams", shading, bounce, n_rays,
+                       d_org_tmin, d_dir_tmax, d_path_id, d_weight, d_out_org_tmin, d_out_dir_tmax, d_out_path_id,
+                       d_sh_org_tmin, d_sh_dir_tmax, d_sh_contrib_pix, d_accum_rgb, skip_shadow_pass=False,
+                       stream=None):
+        """nrt_scene_bake_lightmap_bounce_device: one bounce of BakeLightmap on caller-owned device queues; returns
+        (n_continue, n_shadow)."""
+        nc, ns = C.c_uint64(0), C.c_uint64(0)
+        vp = C.c_void_p
+        opt = lambda x: vp(x) if x else None
+        _check(lib().nrt_scene_bake_lightmap_bounce_device(
+            self._h, vp(d_records_ptr), vp(d_instance_ptr), C.byref(params), C.cast(self._shading(shading), vp),
+            int(bounce), int(n_rays), opt(d_org_tmin), opt(d_dir_tmax), opt(d_path_id), vp(d_weight),
+            vp(d_out_org_tmin), vp(d_out_dir_tmax), vp(d_out_path_id), vp(d_sh_org_tmin), vp(d_sh_dir_tmax),
+            vp(d_sh_contrib_pix), vp(d_accum_rgb), C.byref(nc), C.byref(ns), 1 if skip_shadow_pass else 0,
+            vp(stream) if stream else None))
+        return int(nc.value), int(ns.value)
 
 
 # ------------------------------------------------------------------ BVHAccel<double>

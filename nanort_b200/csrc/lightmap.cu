@@ -25,6 +25,31 @@ int launch_traverse_path_shadow(const Accel *a, const PathQueues &q, const unsig
                                 size_t capacity, float *d_accum, const TraceOptions16 &opt, uint32_t flags,
                                 cudaStream_t s);
 
+// the path pass's parameters of a bake: what path_shade_hit and the slot maps read (also the scene bake's,
+// scene_bake.cu)
+nrt_path_params path_params(const nrt_lightmap_params &lp) {
+  nrt_path_params p = {};
+  p.width = lp.width;
+  p.height = lp.height;
+  p.spp = lp.spp;
+  p.sample0 = lp.sample0;
+  p.seed = lp.seed;
+  p.tile_w = 8;
+  p.tile_h = 4;
+  p.n_shards = 1;
+  p.max_bounces = lp.max_bounces;
+  p.ray_min_t = lp.ray_min_t;
+  p.ray_max_t = lp.ray_max_t;
+  p.n_materials = lp.n_materials;
+  p.n_emissive = lp.n_emissive;
+  p.d_materials = lp.d_materials;
+  p.d_material_ids = lp.d_material_ids;
+  p.d_emissive_faces = lp.d_emissive_faces;
+  p.d_facevarying_normals = lp.d_facevarying_normals;
+  p.flags = lp.flags;
+  return p;
+}
+
 namespace {
 
 // bounce 0 of paths [0, count): continuations to queue `out`, light samples to the shadow queue
@@ -50,30 +75,6 @@ __global__ void next_bounce_kernel(unsigned long long *counters, unsigned long l
   counters[3] = counters[0];
   counters[0] = 0;
   counters[1] = 0;
-}
-
-// the path pass's parameters of a bake: what path_shade_hit and the slot maps read
-nrt_path_params path_params(const nrt_lightmap_params &lp) {
-  nrt_path_params p = {};
-  p.width = lp.width;
-  p.height = lp.height;
-  p.spp = lp.spp;
-  p.sample0 = lp.sample0;
-  p.seed = lp.seed;
-  p.tile_w = 8;
-  p.tile_h = 4;
-  p.n_shards = 1;
-  p.max_bounces = lp.max_bounces;
-  p.ray_min_t = lp.ray_min_t;
-  p.ray_max_t = lp.ray_max_t;
-  p.n_materials = lp.n_materials;
-  p.n_emissive = lp.n_emissive;
-  p.d_materials = lp.d_materials;
-  p.d_material_ids = lp.d_material_ids;
-  p.d_emissive_faces = lp.d_emissive_faces;
-  p.d_facevarying_normals = lp.d_facevarying_normals;
-  p.flags = lp.flags;
-  return p;
 }
 
 int lightmap_check(const Accel *a, const void *d_records, const nrt_lightmap_params *p, const float *d_accum,

@@ -1072,28 +1072,6 @@ void launch_path_camera(const nrt_path_params &p, unsigned long long slot0, uint
 
 namespace {
 
-// One emissive pair in world space, 64 bytes: v0.xyz v1.x | v1.yz v2.xy | v2.z n.xyz | area e.xyz (n: unit
-// cross(e1, e2), area: half its length before normalisation -- geometric_normal() of the world triangle)
-struct SceneLights {
-  const float4 *rec;
-  __device__ __forceinline__ void sample(uint32_t k, float c0, float c1, float c2, float Px, float Py, float Pz,
-                                         float &lx, float &ly, float &lz, float &lnx, float &lny, float &lnz,
-                                         float &area, float &ex, float &ey, float &ez) const {
-    const float4 a = __ldg(rec + 4 * (size_t)k), b = __ldg(rec + 4 * (size_t)k + 1), c = __ldg(rec + 4 * (size_t)k + 2),
-                 d = __ldg(rec + 4 * (size_t)k + 3);
-    lx = c0 * a.x + c1 * a.w + c2 * b.z - Px;
-    ly = c0 * a.y + c1 * b.x + c2 * b.w - Py;
-    lz = c0 * a.z + c1 * b.y + c2 * c.x - Pz;
-    lnx = c.y;
-    lny = c.z;
-    lnz = c.w;
-    area = d.x;
-    ex = d.y;
-    ey = d.z;
-    ez = d.w;
-  }
-};
-
 __global__ void __launch_bounds__(128)
     scene_light_setup_kernel(const uint32_t *__restrict__ pairs, uint32_t n, const InstanceDev *__restrict__ inst,
                              const SceneShadingDev *__restrict__ shading, const PathMaterial *__restrict__ mats,
@@ -1126,10 +1104,12 @@ __global__ void __launch_bounds__(256)
   rays[i] = r;
 }
 
-// the shading of the n radiance rays of queue `in` from their scene hit records
+// the shading of the n radiance rays of queue `in` from their scene hit records; Slots maps a path id to its (pixel
+// or texel, sample): TileSlots for the path pass, TexelSlots for the lightmap bake's bounces 1 and up (scene_bake.cu)
+template <class Slots>
 __global__ void __launch_bounds__(256)
-    scene_path_shade_kernel(nrt_path_params p, unsigned long long slot0, uint32_t bounce, uint32_t n, PathQueues q,
-                            int in, const SceneHit32 *__restrict__ hits, const uint8_t *__restrict__ mask,
+    scene_path_shade_kernel(nrt_path_params p, Slots slots, uint32_t bounce, uint32_t n, PathQueues q, int in,
+                            const SceneHit32 *__restrict__ hits, const uint8_t *__restrict__ mask,
                             const InstanceDev *__restrict__ inst, const float *__restrict__ state76,
                             const SceneShadingDev *__restrict__ shading, const float4 *__restrict__ lights,
                             float *accum, unsigned long long *counters) {
@@ -1139,8 +1119,7 @@ __global__ void __launch_bounds__(256)
   uint32_t pid = 0, pix, smp;
   if (i < n && mask[i]) {
     pid = q.path_id[in][i];
-    if (slot_to_pixel(tile_map(p), slot0 + pid, pix, smp)) {
-      smp += p.sample0;
+    if (slots(p, pid, pix, smp)) {
       const float4 o = q.org_tmin[in][i], d = q.dir_tmax[in][i];
       const SceneHit32 h = hits[i];
       const SceneShadingDev sh = shading[h.node_id];
@@ -1193,46 +1172,22 @@ __global__ void __launch_bounds__(256)
   atomicAdd(accum + 3 * pix + 2, c.z);
 }
 
-// What one call owns on the device: the per-instance shading table, the light records and the walk's buffers.
-struct ScenePathCall {
-  Scene *sc = nullptr;
-  nrt_path_params p{};
-  uint32_t trav_flags = 0;
-  SceneShadingDev *shading = nullptr;
-  float4 *lights = nullptr;
-  Ray36 *rays = nullptr;
-  SceneHit32 *hits = nullptr;
-  uint8_t *mask = nullptr;
-  unsigned long long *ctr = nullptr;  // [0] continuation rays, [1] shadow rays, [2] camera rays
-  uint32_t launches = 0, trav_launches = 0;
-  ~ScenePathCall() {
-    cudaFree(shading), cudaFree(lights), cudaFree(rays), cudaFree(hits), cudaFree(mask), cudaFree(ctr);
-  }
-};
+}  // namespace
 
-// Checks the arguments (nothing is launched when they are refused), reads the emissive pairs back, allocates the
-// call's buffers for `cap` rays and writes the shading table and the light records.
-int scene_path_begin(const char *name, const nrt_scene *s, const nrt_path_params *pp, const nrt_scene_shading *shading,
+int scene_path_setup(const char *name, const nrt_scene *s, const nrt_path_params &p, const nrt_scene_shading *shading,
                      size_t cap, cudaStream_t st, ScenePathCall &c) {
   auto refuse = [&](const char *why) {
     set_error(std::string(name) + ": " + why);
     return NRT_ERR_INVALID;
   };
-  if (!s || !pp) return refuse("NULL argument");
   if (!shading) return refuse("NULL shading array (one nrt_scene_shading per instance)");
-  const nrt_path_params p = *pp;
-  if (p.width == 0 || p.height == 0 || p.spp == 0 || p.n_shards == 0 || p.shard >= p.n_shards || p.tile_w == 0 ||
-      p.tile_h == 0 || (p.tile_w % 8) != 0 || (p.tile_h % 4) != 0 || p.max_bounces == 0 || p.n_materials == 0 ||
-      !p.d_materials || (p.n_emissive > 0 && !p.d_emissive_faces))
-    return refuse("bad parameters");
   if (p.d_material_ids || p.d_facevarying_normals)
     return refuse("material ids and face-varying normals are given per instance (nrt_scene_shading), not in the params");
   if (p.flags & NRT_TRAVERSE_ANY_HIT) return refuse("NRT_TRAVERSE_ANY_HIT is not supported by the scene walk");
-  if (p.flags & NRT_AO_PACKED_TILES) return refuse("NRT_AO_PACKED_TILES is not supported");
   Scene *sc = const_cast<Scene *>(reinterpret_cast<const Scene *>(s));
   for (uint32_t i = 0; i < sc->n; i++)
     if (sc->n_faces[i] == 0) return refuse("triangle instances only");
-  c.sc = sc;
+  c.s = s;
   c.p = p;
   c.trav_flags = p.flags & 0xFFFFu;
   std::vector<uint32_t> pairs(2 * (size_t)p.n_emissive);
@@ -1250,8 +1205,9 @@ int scene_path_begin(const char *name, const nrt_scene *s, const nrt_path_params
   if (p.n_emissive && cap > 0) {
     NRT_CUDA(cudaMalloc(&c.lights, 4 * sizeof(float4) * p.n_emissive));
     scene_light_setup_kernel<<<(p.n_emissive + 127) / 128, 128, 0, st>>>(
-        static_cast<const uint32_t *>(p.d_emissive_faces), p.n_emissive, sc->d_inst, c.shading,
-        static_cast<const PathMaterial *>(p.d_materials), c.lights);
+        static_cast<const uint32_t *>(p.d_emissive_faces), p.n_emissive, sc->d_inst,
+        c.shading, static_cast<const PathMaterial *>(p.d_materials),
+        c.lights);
     NRT_CUDA(cudaGetLastError());
     c.launches++;
   }
@@ -1263,35 +1219,76 @@ int scene_path_begin(const char *name, const nrt_scene *s, const nrt_path_params
   return NRT_OK;
 }
 
-// One bounce: walk the n rays of queue `in`, shade them, read the counts; then walk the shadow rays and add the
-// visible light samples.  out[0] continuation rays, out[1] shadow rays, out[2] camera rays (ctr[2]).
-int scene_path_bounce(ScenePathCall &c, unsigned long long slot0, uint32_t bounce, uint32_t n, const PathQueues &q,
-                      int in, float *accum, bool shadow_pass, unsigned long long out[3], cudaStream_t st) {
+// The shadow walk of a bounce: walk the ns rays of the shadow queue and add the visible light samples.
+int scene_shadow_pass(ScenePathCall &c, const PathQueues &q, uint32_t ns, float *accum, cudaStream_t st) {
+  if (ns == 0) return NRT_OK;
+  Scene *sc = const_cast<Scene *>(reinterpret_cast<const Scene *>(c.s));
+  const unsigned sb = (ns + 255) / 256;
+  SceneHit32 *hits = c.hits;
+  scene_pack_rays_kernel<<<sb, 256, 0, st>>>(q.sh_org_tmin, q.sh_dir_tmax, ns, c.rays);
+  if (const int rc = scene_launch(sc, c.rays, ns, hits, c.mask, c.trav_flags, st)) return rc;
+  scene_path_shadow_kernel<<<sb, 256, 0, st>>>(hits, c.mask, q.sh_dir_tmax, q.sh_contrib_pix, ns, accum);
+  NRT_CUDA(cudaGetLastError());
+  c.launches += 3;
+  c.trav_launches += 1;
+  return NRT_OK;
+}
+
+namespace {
+
+// Checks the path pass's own parameters (nothing is launched when they are refused), then scene_path_setup.
+int scene_path_begin(const char *name, const nrt_scene *s, const nrt_path_params *pp, const nrt_scene_shading *shading,
+                     size_t cap, cudaStream_t st, ScenePathCall &c) {
+  auto refuse = [&](const char *why) {
+    set_error(std::string(name) + ": " + why);
+    return NRT_ERR_INVALID;
+  };
+  if (!s || !pp) return refuse("NULL argument");
+  const nrt_path_params p = *pp;
+  if (p.width == 0 || p.height == 0 || p.spp == 0 || p.n_shards == 0 || p.shard >= p.n_shards || p.tile_w == 0 ||
+      p.tile_h == 0 || (p.tile_w % 8) != 0 || (p.tile_h % 4) != 0 || p.max_bounces == 0 || p.n_materials == 0 ||
+      !p.d_materials || (p.n_emissive > 0 && !p.d_emissive_faces))
+    return refuse("bad parameters");
+  if (p.flags & NRT_AO_PACKED_TILES) return refuse("NRT_AO_PACKED_TILES is not supported");
+  return scene_path_setup(name, s, p, shading, cap, st, c);
+}
+
+// One bounce: walk the n rays of queue `in`, shade them (Slots: TileSlots or TexelSlots), read the counts;
+// then, with shadow_pass, walk the shadow rays and add the visible light samples.  out[0] continuation rays, out[1]
+// shadow rays, out[2] camera rays (ctr[2]).
+template <class Slots>
+int scene_bounce(ScenePathCall &c, const Slots &slots, uint32_t bounce, uint32_t n, const PathQueues &q, int in,
+                 float *accum, bool shadow_pass, unsigned long long out[3], cudaStream_t st) {
+  Scene *sc = const_cast<Scene *>(reinterpret_cast<const Scene *>(c.s));
   const unsigned blocks = (n + 255) / 256;
+  SceneHit32 *hits = c.hits;
   NRT_CUDA(cudaMemsetAsync(c.ctr, 0, 2 * sizeof(unsigned long long), st));
   scene_pack_rays_kernel<<<blocks, 256, 0, st>>>(q.org_tmin[in], q.dir_tmax[in], n, c.rays);
-  if (const int rc = scene_launch(c.sc, c.rays, n, c.hits, c.mask, c.trav_flags, st)) return rc;
-  scene_path_shade_kernel<<<blocks, 256, 0, st>>>(c.p, slot0, bounce, n, q, in, c.hits, c.mask, c.sc->d_inst,
-                                                  c.sc->d_state, c.shading, c.lights, accum, c.ctr);
+  if (const int rc = scene_launch(sc, c.rays, n, hits, c.mask, c.trav_flags, st)) return rc;
+  scene_path_shade_kernel<<<blocks, 256, 0, st>>>(c.p, slots, bounce, n, q, in, hits, c.mask, sc->d_inst,
+                                                  sc->d_state, c.shading,
+                                                  c.lights, accum, c.ctr);
   NRT_CUDA(cudaGetLastError());
   NRT_CUDA(cudaMemcpyAsync(out, c.ctr, 3 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
   NRT_CUDA(cudaStreamSynchronize(st));  // the scene walk takes its ray count from the host
   c.launches += 3;
   c.trav_launches += 1;
-  const uint32_t ns = (uint32_t)out[1];
-  if (shadow_pass && ns > 0) {
-    const unsigned sb = (ns + 255) / 256;
-    scene_pack_rays_kernel<<<sb, 256, 0, st>>>(q.sh_org_tmin, q.sh_dir_tmax, ns, c.rays);
-    if (const int rc = scene_launch(c.sc, c.rays, ns, c.hits, c.mask, c.trav_flags, st)) return rc;
-    scene_path_shadow_kernel<<<sb, 256, 0, st>>>(c.hits, c.mask, q.sh_dir_tmax, q.sh_contrib_pix, ns, accum);
-    NRT_CUDA(cudaGetLastError());
-    c.launches += 3;
-    c.trav_launches += 1;
-  }
-  return NRT_OK;
+  return shadow_pass ? scene_shadow_pass(c, q, (uint32_t)out[1], accum, st) : NRT_OK;
+}
+
+int scene_path_bounce(ScenePathCall &c, unsigned long long slot0, uint32_t bounce, uint32_t n, const PathQueues &q,
+                      int in, float *accum, bool shadow_pass, unsigned long long out[3], cudaStream_t st) {
+  return scene_bounce(c, TileSlots{slot0}, bounce, n, q, in, accum, shadow_pass, out, st);
 }
 
 }  // namespace
+
+// Bounces 1 and up of the scene lightmap bake (scene_bake.cu): scene_bounce with the texel slot map.
+int scene_texel_bounce(ScenePathCall &c, const TexelSlots &slots, uint32_t bounce, uint32_t n, const PathQueues &q,
+                       int in, float *accum, bool shadow_pass, unsigned long long out[3], cudaStream_t st) {
+  return scene_bounce(c, slots, bounce, n, q, in, accum, shadow_pass, out, st);
+}
+
 }  // namespace nrt
 
 extern "C" int nrt_scene_render_path_device(const nrt_scene *s, const nrt_path_params *pp,

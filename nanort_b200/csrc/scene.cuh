@@ -1,12 +1,28 @@
-// Device-side pieces of the two-level scene shared by scene.cu's passes and bdpt.cu's scene pass: the instance record,
-// the scene walk's hit record, Matrix::MultV, world-space triangles and normals, the rule that lifts spawned rays off
-// a surface, and the host entry points bdpt.cu walks the scene through.
+// Device-side pieces of the two-level scene shared by scene.cu's passes, bdpt.cu's scene pass and scene_bake.cu's
+// bakes: the instance record, the scene walk's hit record, Matrix::MultV, world-space triangles, normals and light
+// records, the rule that lifts spawned rays off a surface, and the host entry points the other files walk the scene
+// and run the path pass's stages through.
 #pragma once
 
 #include "../../include/nanort_b200_scene_path.h"
 #include "common.cuh"
 
 namespace nrt {
+
+// the scene walk's hit record and one instance's shading inputs (named outside the anonymous namespace below, so
+// that ScenePathCall can hold them typed)
+struct SceneHit32 {
+  float u, v, t;
+  uint32_t prim_id, node_id;
+  float P[3];
+};
+static_assert(sizeof(SceneHit32) == 32, "nrt_scene_hit");
+
+struct SceneShadingDev {  // nrt_scene_shading
+  const uint32_t *mat_ids;
+  const float *fvn;
+};
+static_assert(sizeof(SceneShadingDev) == sizeof(nrt_scene_shading), "nrt_scene_shading");
 
 namespace {
 
@@ -36,13 +52,6 @@ struct SceneDev {
   const PackedTri *top_slots;  // its leaves: {world bmin, instance id | world bmax, last flag | -}
 };
 
-struct SceneHit32 {
-  float u, v, t;
-  uint32_t prim_id, node_id;
-  float P[3];
-};
-static_assert(sizeof(SceneHit32) == 32, "nrt_scene_hit");
-
 // t[k] = ((m[0][k] v0 + m[1][k] v1) + m[2][k] v2) + m[3][k]   (Matrix::MultV, nanosg.h:214-222)
 __device__ __forceinline__ void multv(const Mat43 &m, float x, float y, float z, float &ox, float &oy, float &oz) {
   ox = ((m.a.x * x + m.a.w * y) + m.b.z * z) + m.c.y;
@@ -58,12 +67,6 @@ __device__ __forceinline__ Mat43 load_mat(const Mat43 *p) {
   m.c = __ldg(q + 2);
   return m;
 }
-
-struct SceneShadingDev {  // nrt_scene_shading
-  const uint32_t *mat_ids;
-  const float *fvn;
-};
-static_assert(sizeof(SceneShadingDev) == sizeof(nrt_scene_shading), "nrt_scene_shading");
 
 // Spawned rays start lift = ray_min_t above P along the unit geometric normal g, on the side the ray leaves.
 struct SceneSpawn {
@@ -139,6 +142,27 @@ __device__ __forceinline__ void world_normal(const float w[9], float &nx, float 
   nz *= il;
 }
 
+// One emissive pair in world space, 64 bytes: v0.xyz v1.x | v1.yz v2.xy | v2.z n.xyz | area e.xyz (n: unit
+// cross(e1, e2), area: half its length before normalisation -- geometric_normal() of the world triangle)
+struct SceneLights {
+  const float4 *rec;
+  __device__ __forceinline__ void sample(uint32_t k, float c0, float c1, float c2, float Px, float Py, float Pz,
+                                         float &lx, float &ly, float &lz, float &lnx, float &lny, float &lnz,
+                                         float &area, float &ex, float &ey, float &ez) const {
+    const float4 a = __ldg(rec + 4 * (size_t)k), b = __ldg(rec + 4 * (size_t)k + 1), c = __ldg(rec + 4 * (size_t)k + 2),
+                 d = __ldg(rec + 4 * (size_t)k + 3);
+    lx = c0 * a.x + c1 * a.w + c2 * b.z - Px;
+    ly = c0 * a.y + c1 * b.x + c2 * b.w - Py;
+    lz = c0 * a.z + c1 * b.y + c2 * c.x - Pz;
+    lnx = c.y;
+    lny = c.z;
+    lnz = c.w;
+    area = d.x;
+    ex = d.y;
+    ey = d.z;
+    ez = d.w;
+  }
+};
 
 }  // namespace
 
@@ -156,5 +180,29 @@ SceneView scene_view(const nrt_scene *s);
 // earlier walks of the scene that used the same scratch
 int scene_walk(const nrt_scene *s, const Ray36 *d_rays, size_t n, void *d_hits, uint8_t *d_mask, uint32_t flags,
                cudaStream_t st);
+
+// What one scene path or lightmap call owns on the device: the per-instance shading table, the world-space light
+// records (SceneLights) and the walk's buffers.
+struct ScenePathCall {
+  const nrt_scene *s = nullptr;
+  nrt_path_params p{};
+  uint32_t trav_flags = 0;
+  SceneShadingDev *shading = nullptr;
+  float4 *lights = nullptr;
+  Ray36 *rays = nullptr;
+  SceneHit32 *hits = nullptr;
+  uint8_t *mask = nullptr;
+  unsigned long long *ctr = nullptr;  // [0] continuation rays, [1] shadow rays, [2] camera rays
+  uint32_t launches = 0, trav_launches = 0;
+  ~ScenePathCall() {
+    cudaFree(shading), cudaFree(lights), cudaFree(rays), cudaFree(hits), cudaFree(mask), cudaFree(ctr);
+  }
+};
+// The set-up both scene.cu's path pass and the scene lightmap bake start with, after their own parameter checks:
+// refuses a NULL shading array, material ids or normals in p, ANY_HIT, a non-triangle instance and an emissive pair
+// that is no {instance, face} of the scene (read back once); then allocates the call's buffers for `cap` rays and
+// writes the shading table and the light records.
+int scene_path_setup(const char *name, const nrt_scene *s, const nrt_path_params &p, const nrt_scene_shading *shading,
+                     size_t cap, cudaStream_t st, ScenePathCall &c);
 
 }  // namespace nrt
