@@ -10,6 +10,7 @@
 #include "common.cuh"
 #include "scan.cuh"
 #include "wavefront.cuh"
+#include "pass_host.cuh"
 
 namespace nrt {
 
@@ -79,16 +80,27 @@ bool is_triangle_accel(const Accel *a) {
   return a->prim_kind == 0 && !a->d_prim_boxes && a->d_faces && a->d_verts && a->d_pair && a->d_tris_cm;
 }
 
+// The covered-texel compaction of n records: flags, then offsets, the list of covered texels and the scan's scratch.
+// The flat bakes keep it at the start of the accel's pass scratch, the scene bakes in their call's memory.
+Compaction carve_compaction(Carver &c, uint32_t n) {
+  Compaction r;
+  r.offs = c.take<uint32_t>(n);
+  r.list = c.take<uint32_t>(n);
+  r.scratch = c.take<uint32_t>(scan_scratch_words(n));
+  return r;
+}
+
 // Compacts the covered texels of the n records into `list` and reads their count back, under the world accel's pass
-// ordering, which the caller holds; d_wave holds at least (2 n + scan_scratch_words(n)) words.  Refuses (after the
-// compaction's launches, before any traversal) records whose prim_id is neither a miss nor a face of `a`.  The AO
-// bake and the lightmap bake (lightmap.cu) start here.
+// ordering, which the caller holds; d_wave starts with carve_compaction(n).  Refuses (after the compaction's launches,
+// before any traversal) records whose prim_id is neither a miss nor a face of `a`.  The AO bake and the lightmap bake
+// (lightmap.cu) start here.
 int bake_prepare(Accel *a, const void *d_records, uint32_t n, const char *who, cudaStream_t s, uint32_t **list,
                  uint32_t *n_cov, uint32_t *launches) {
-  uint32_t *offs = static_cast<uint32_t *>(a->d_wave);
-  *list = offs + n;
-  uint32_t *scratch = *list + n;
-  unsigned long long *info = reinterpret_cast<unsigned long long *>(a->d_counters) + 2;  // [2] covered, [3] bad record
+  Carver c(a->d_wave);
+  const Compaction cp = carve_compaction(c, n);
+  uint32_t *offs = cp.offs, *scratch = cp.scratch;
+  *list = cp.list;
+  unsigned long long *info = pass_counters(a, kWaveCounters);  // [2] covered, [3] bad record
   const Hit16 *rec = static_cast<const Hit16 *>(d_records);
   NRT_CUDA(cudaMemsetAsync(info, 0, 2 * sizeof(unsigned long long), s));
   covered_flags_kernel<<<(n + 255) / 256, 256, 0, s>>>(rec, n, a->n_prims, offs, info);
@@ -161,7 +173,7 @@ extern "C" int nrt_uv_raster_device(const nrt_accel *uv_h, const nrt_accel *worl
   if (conf) {
     if (const int rc = grow_wave(a, (size_t)n * sizeof(Hit16))) return rc;
   }
-  unsigned long long *covered = reinterpret_cast<unsigned long long *>(a->d_counters) + 2;
+  unsigned long long *covered = pass_counters(a, kWaveCounters);
   NRT_CUDA(cudaMemsetAsync(covered, 0, sizeof(unsigned long long), s));
 
   TexelRays rays;
@@ -201,11 +213,7 @@ static int bake_check(const Accel *a, const void *d_records, const nrt_bake_para
     set_error(std::string(who) + ": NULL argument");
     return NRT_ERR_INVALID;
   }
-  const uint64_t n = (uint64_t)p->width * p->height;
-  if (n == 0 || n > kMaxTexels || p->spp == 0) {
-    set_error(std::string(who) + ": width * height must lie in [1, 2^31] and spp must be positive");
-    return NRT_ERR_INVALID;
-  }
+  if (const int rc = check_bake_params(*p, who)) return rc;
   if (p->flags & ~(uint32_t)(NRT_TRAVERSE_ANY_HIT | NRT_TRAVERSE_CPP03_INVERSE)) {
     set_error(std::string(who) + ": flags other than NRT_TRAVERSE_ANY_HIT / NRT_TRAVERSE_CPP03_INVERSE "
                                  "(the conformance walk is not offered: export the rays and trace them with it)");
@@ -257,26 +265,12 @@ static int run_bake(const nrt_accel *h, const void *d_records, const nrt_bake_pa
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (const int rc = wait_previous_pass(a, s)) return rc;
   const RecordOnExit pass_done{a->pass_done, s};
-  if (const int rc = grow_wave(a, (2 * (size_t)n + scan_scratch_words(n)) * sizeof(uint32_t))) return rc;
+  if (const int rc = carve_pass_scratch(a, [&](Carver &c) { carve_compaction(c, n); })) return rc;
   uint32_t launches = a->d_face_n ? 0u : 1u;
   if (const int rc = ensure_face_normals(a, s)) return rc;
 
-  cudaEvent_t e_begin = nullptr, e_end = nullptr;
-  std::vector<cudaEvent_t> ev;
-  struct Events {  // destroyed on every exit
-    std::vector<cudaEvent_t> &v;
-    ~Events() {
-      for (cudaEvent_t e : v)
-        if (e) cudaEventDestroy(e);
-    }
-  } events{ev};
-  if (res) {
-    NRT_CUDA(cudaEventCreate(&e_begin));
-    ev.push_back(e_begin);
-    NRT_CUDA(cudaEventCreate(&e_end));
-    ev.push_back(e_end);
-    NRT_CUDA(cudaEventRecord(e_begin, s));
-  }
+  PassClock clock(res != nullptr);
+  if (const int rc = clock.start(s)) return rc;
   uint32_t *list = nullptr, n_cov = 0;
   if (const int rc = bake_prepare(a, d_records, n, who, s, &list, &n_cov, &launches)) return rc;
   const uint64_t total = (uint64_t)n_cov * p.spp;
@@ -285,7 +279,7 @@ static int run_bake(const nrt_accel *h, const void *d_records, const nrt_bake_pa
     set_error(std::string(who) + ": the ray buffer holds fewer records than covered texels x spp");
     return NRT_ERR_INVALID;
   }
-  unsigned long long *occluded = reinterpret_cast<unsigned long long *>(a->d_counters) + 4;
+  unsigned long long *occluded = pass_counters(a, kPassTotals);
   NRT_CUDA(cudaMemsetAsync(occluded, 0, sizeof(unsigned long long), s));
   uint32_t trav_launches = 0;
   if (n_cov > 0) {
@@ -301,36 +295,24 @@ static int run_bake(const nrt_accel *h, const void *d_records, const nrt_bake_pa
         launches++;
         continue;
       }
-      cudaEvent_t t0 = nullptr, t1 = nullptr;
-      if (res) {
-        NRT_CUDA(cudaEventCreate(&t0));
-        ev.push_back(t0);
-        NRT_CUDA(cudaEventCreate(&t1));
-        ev.push_back(t1);
-        NRT_CUDA(cudaEventRecord(t0, s));
-      }
+      if (const int rc = clock.begin(s)) return rc;
       if (const int rc = launch_traverse_bake(a, rays, count, d_accum, occluded, p.flags, s)) return rc;
-      if (res) NRT_CUDA(cudaEventRecord(t1, s));
+      if (const int rc = clock.end(s)) return rc;
       launches++;
       trav_launches++;
     }
   }
   if (res) {
     unsigned long long hits = 0;
-    NRT_CUDA(cudaEventRecord(e_end, s));
+    if (const int rc = clock.stop(s)) return rc;
     NRT_CUDA(cudaMemcpyAsync(&hits, occluded, sizeof(hits), cudaMemcpyDeviceToHost, s));
     NRT_CUDA(cudaStreamSynchronize(s));
-    float tms = 0.0f, total_ms = 0.0f;
-    for (size_t i = 2; i + 1 < ev.size(); i += 2) {
-      float m = 0.0f;
-      NRT_CUDA(cudaEventElapsedTime(&m, ev[i], ev[i + 1]));
-      tms += m;
-    }
-    NRT_CUDA(cudaEventElapsedTime(&total_ms, e_begin, e_end));
+    float total_ms = 0.0f, span[2];
+    if (const int rc = clock.read(&total_ms, span)) return rc;
     res->texels = n_cov;
     res->ao_rays = total;
     res->ao_hits = hits;
-    res->traverse_ms = tms;
+    res->traverse_ms = span[0];
     res->total_ms = total_ms;
     res->launches = launches;
     res->traverse_launches = trav_launches;

@@ -14,6 +14,7 @@
 #include "scan.cuh"
 #include "scene.cuh"
 #include "wavefront.cuh"
+#include "pass_host.cuh"
 
 namespace nrt {
 
@@ -652,99 +653,102 @@ struct Out {  // export buffers (nullptr: render into accum)
 
 // the rules both passes share
 int check_common(const nrt_bdpt_params &p, const char *who) {
-  auto bad = [&](const char *why) {
-    set_error(std::string(who) + ": " + why);
-    return NRT_ERR_INVALID;
-  };
   if (p.flags & ~(uint32_t)NRT_TRAVERSE_CONFORMANCE)
-    return bad("flags other than NRT_TRAVERSE_CONFORMANCE (calcG needs the nearest distance: no ANY_HIT)");
+    return refuse(who,
+                  "flags other than NRT_TRAVERSE_CONFORMANCE (calcG needs the nearest distance: no ANY_HIT)");
   if (p.width == 0 || p.height == 0 || p.spp == 0 || p.n_shards == 0 || p.shard >= p.n_shards || p.tile_w == 0 ||
       p.tile_h == 0 || (p.tile_w % 8) != 0 || (p.tile_h % 4) != 0)
-    return bad("bad image, sample or tile parameters");
-  if ((uint64_t)p.sample0 + p.spp > p.spp_total) return bad("sample0 + spp > spp_total");
-  if (p.max_bounces == 0 || p.max_bounces > 64) return bad("max_bounces must lie in [1, 64]");
+    return refuse(who, "bad image, sample or tile parameters");
+  if ((uint64_t)p.sample0 + p.spp > p.spp_total) return refuse(who, "sample0 + spp > spp_total");
+  if (p.max_bounces == 0 || p.max_bounces > 64) return refuse(who, "max_bounces must lie in [1, 64]");
   return NRT_OK;
 }
 
 int check_params(const Accel *a, const nrt_bdpt_params *pp, const char *who) {
-  auto bad = [&](const char *why) {
-    set_error(std::string(who) + ": " + why);
-    return NRT_ERR_INVALID;
-  };
-  if (!a || !pp) return bad("NULL argument");
+  if (!a || !pp) return refuse(who, "NULL argument");
   const nrt_bdpt_params &p = *pp;
   if (!p.d_materials || !p.d_material_ids || !p.d_facevarying_normals || p.n_materials == 0)
-    return bad("materials, material ids and face-varying normals are required");
+    return refuse(who, "materials, material ids and face-varying normals are required");
   if (const int rc = check_common(p, who)) return rc;
   if (a->prim_kind != 0 || a->d_prim_boxes || !a->d_faces || !a->d_verts || !a->d_pair || !a->d_tris_cm)
-    return bad("the accel must be a triangle accel");
+    return refuse(who, "the accel must be a triangle accel");
   return NRT_OK;
 }
 
-size_t rnd256(size_t x) { return (x + 255) & ~(size_t)255; }
-
-// Sizes of one call: this shard's slots, the wave capacity and the scratch of the light table and of one wave.
+// Sizes of one call: this shard's slots, the wave capacity and the light table's capacity.
 // extra_per_slot: what a pass keeps per slot beyond the flat pass's records.
 struct Layout {
   TileMap tm;
   unsigned long long total_slots, cap;
   uint32_t B, stride, mc, n_lights_max;  // n_lights_max: faces (flat) or pairs (scene)
-  size_t light_bytes, wave_bytes;
+  bool exported;
 };
 
 int make_layout(const nrt_bdpt_params &p, bool exported, uint32_t nf, size_t extra_per_slot, const char *who,
                 Layout &L) {
   L.tm = TileMap{p.width, p.height, p.spp, p.sample0, p.tile_w, p.tile_h, p.shard, p.n_shards, 0u};
-  const uint32_t tiles_x = (p.width + p.tile_w - 1) / p.tile_w, tiles_y = (p.height + p.tile_h - 1) / p.tile_h;
-  const uint32_t n_tiles = tiles_x * tiles_y;
-  const uint32_t my_tiles = n_tiles > p.shard ? (n_tiles - p.shard + p.n_shards - 1) / p.n_shards : 0;
-  const unsigned long long per_tile = (unsigned long long)p.tile_w * p.tile_h * p.spp;
-  L.total_slots = (unsigned long long)my_tiles * per_tile;
+  const ShardSlots sh = shard_slots(p.width, p.height, p.tile_w, p.tile_h, p.spp, p.shard, p.n_shards);
+  L.total_slots = sh.total;
   L.B = p.max_bounces;
   L.stride = L.B + 1;
   L.mc = max_conns(L.B);
+  L.exported = exported;
   const uint32_t stride = L.stride, mc = L.mc;
   // per slot: state, two subpaths (unless exported), queues, counts, offsets, emission, colour, records
   const size_t per_slot = sizeof(PathState) + (exported ? 0 : 2 * (size_t)stride * sizeof(nrt_bdpt_vertex) + 8 + 12) +
                           2 * 4 + 4 + 4 + 12 + (size_t)mc * sizeof(Conn) + 8 + extra_per_slot;
-  unsigned long long tiles_per_wave = kWaveBudget / (per_slot * per_tile);
-  if (tiles_per_wave == 0) tiles_per_wave = 1;
-  const unsigned long long cap = std::min<unsigned long long>(L.total_slots, tiles_per_wave * per_tile);
-  L.cap = cap;
-  if (cap > 0xFFFFFFFFull / mc) {
+  L.cap = sh.wave(kWaveBudget / per_slot);
+  if (L.cap > 0xFFFFFFFFull / mc) {
     set_error(std::string(who) + ": a tile holds too many samples");
     return NRT_ERR_INVALID;
   }
   L.n_lights_max = nf;
-  const uint32_t sort_tiles = (nf + kSortTile - 1) / kSortTile;
-  L.light_bytes = 5 * rnd256(4 * (size_t)nf) + rnd256(4 * (16 * (size_t)sort_tiles + 1)) +
-                  rnd256(4 * std::max(scan_scratch_words(nf), scan_scratch_words(16 * sort_tiles))) + rnd256(16);
-  L.wave_bytes = rnd256(cap * sizeof(PathState)) +
-                 (exported ? 0 : 2 * rnd256(cap * stride * sizeof(nrt_bdpt_vertex)) + 2 * rnd256(cap * 4) + rnd256(cap * 12)) +
-                 4 * rnd256(cap * 4) + rnd256(cap * 12) + rnd256(cap * mc * sizeof(Conn)) +
-                 rnd256(scan_scratch_words((uint32_t)cap) * 4);
   return NRT_OK;
 }
 
-// CUDA events around the traversal launches (res != NULL)
-struct Timer {
-  std::vector<cudaEvent_t> &ev;
-  bool on;
-  int begin(cudaStream_t s) {
-    if (!on) return NRT_OK;
-    cudaEvent_t t0 = nullptr, t1 = nullptr;
-    NRT_CUDA(cudaEventCreate(&t0));
-    ev.push_back(t0);
-    NRT_CUDA(cudaEventCreate(&t1));
-    ev.push_back(t1);
-    NRT_CUDA(cudaEventRecord(t0, s));
-    return NRT_OK;
-  }
-  int end(cudaStream_t s) {
-    if (on) NRT_CUDA(cudaEventRecord(ev.back(), s));
-    return NRT_OK;
-  }
+// The scratch of one pass: the light table, then the buffers of one wave
+struct Scratch {
+  uint32_t *l_flags, *l_offs, *l_ids, *l_keys, *l_keys_tmp, *l_table, *l_scratch;
+  float *l_total;
+  PathState *st;
+  nrt_bdpt_vertex *w_eye, *w_light;  // the wave's subpaths, their lengths and the sample colours (not exported)
+  uint32_t *w_ne, *w_nl;
+  float *w_rgb;
+  uint32_t *queue[2], *cnt, *offs;
+  float3 *emit;
+  Conn *conns;
+  uint32_t *scan_scratch;
 };
+
+Scratch carve_scratch(Carver &c, const Layout &L) {
+  const uint32_t nf = L.n_lights_max, sort_tiles = (nf + kSortTile - 1) / kSortTile;
+  const size_t cap = L.cap;
+  Scratch m = {};
+  m.l_flags = c.take<uint32_t>(nf);
+  m.l_offs = c.take<uint32_t>(nf);
+  m.l_ids = c.take<uint32_t>(nf);
+  m.l_keys = c.take<uint32_t>(nf);
+  m.l_keys_tmp = c.take<uint32_t>(nf);
+  m.l_table = c.take<uint32_t>(16 * (size_t)sort_tiles + 1);
+  m.l_scratch = c.take<uint32_t>(std::max(scan_scratch_words(nf), scan_scratch_words(16 * sort_tiles)));
+  m.l_total = c.take<float>(4);
+  m.st = c.take<PathState>(cap);
+  if (!L.exported) {
+    m.w_eye = c.take<nrt_bdpt_vertex>(cap * L.stride);
+    m.w_light = c.take<nrt_bdpt_vertex>(cap * L.stride);
+    m.w_ne = c.take<uint32_t>(cap);
+    m.w_nl = c.take<uint32_t>(cap);
+    m.w_rgb = c.take<float>(3 * cap);
+  }
+  m.queue[0] = c.take<uint32_t>(cap);
+  m.queue[1] = c.take<uint32_t>(cap);
+  m.cnt = c.take<uint32_t>(cap);
+  m.offs = c.take<uint32_t>(cap);
+  m.emit = c.take<float3>(cap);
+  m.conns = c.take<Conn>(cap * L.mc);
+  m.scan_scratch = c.take<uint32_t>(scan_scratch_words((uint32_t)cap));
+  return m;
+}
 
 // The flat mesh: the light table over its faces, the accel's traversal launches with the retire steps
 struct FlatWalk {
@@ -768,7 +772,7 @@ struct FlatWalk {
   // ctr[0]: the launch's rays (device); ctr[1] receives the continuing ones.  The count stays on the device, so
   // *empty (no ray left: the later bounces of this subpath can be skipped) is never known here.
   int bounce(const Scene &sc, const Subpaths &sp, PathState *st, const uint32_t *q_in, uint32_t *q_out,
-             unsigned long long *ctr, uint32_t count, uint32_t B, int eye, Timer &tm, uint32_t &launches,
+             unsigned long long *ctr, uint32_t count, uint32_t B, int eye, PassClock &tm, uint32_t &launches,
              uint32_t &trav_launches, bool *empty, cudaStream_t s) {
     *empty = false;
     if (const int rc = tm.begin(s)) return rc;
@@ -780,7 +784,7 @@ struct FlatWalk {
     trav_launches++;
     return NRT_OK;
   }
-  int connect(Conn *conns, const Subpaths &sp, unsigned long long *ctr, size_t capacity, Timer &tm,
+  int connect(Conn *conns, const Subpaths &sp, unsigned long long *ctr, size_t capacity, PassClock &tm,
               uint32_t &launches, uint32_t &trav_launches, cudaStream_t s) {
     if (const int rc = tm.begin(s)) return rc;
     if (const int rc = launch_traverse_bdpt_connect(a, ConnRays{conns, sp}, ConnEpilogue{conns, sp}, ctr, capacity,
@@ -793,59 +797,30 @@ struct FlatWalk {
   }
 };
 
-// One pass over L's slots on the scratch at `b`: the light table, then per wave eye starts, eye bounces, light starts,
+// One pass over L's slots on the scratch m: the light table, then per wave eye starts, eye bounces, light starts,
 // light bounces, the connection records, the connection walk and the sums.  `cnt64` holds the pass's counters
 // ([0, 2) light table info, [2, 4) queue counts, [4, 7) ray totals).
 template <class Walk>
-int run_pass(Walk &wk, const nrt_bdpt_params &p, const Layout &L, Scene sc, char *b, unsigned long long *info,
+int run_pass(Walk &wk, const nrt_bdpt_params &p, const Layout &L, Scene sc, const Scratch &m, unsigned long long *info,
              unsigned long long *ctr, unsigned long long *totals, float *d_accum, const Out *out, nrt_bdpt_result *res,
              cudaStream_t s, const char *who) {
   const TileMap tm = L.tm;
   const unsigned long long total_slots = L.total_slots, cap = L.cap;
   const uint32_t B = L.B, stride = L.stride, mc = L.mc, nf = L.n_lights_max;
-  const uint32_t sort_tiles = (nf + kSortTile - 1) / kSortTile;
-  auto take = [&](size_t bytes) {
-    char *r = b;
-    b += rnd256(bytes);
-    return r;
-  };
-  // light table
-  uint32_t *l_flags = reinterpret_cast<uint32_t *>(take(4 * (size_t)nf));
-  uint32_t *l_offs = reinterpret_cast<uint32_t *>(take(4 * (size_t)nf));
-  uint32_t *l_ids = reinterpret_cast<uint32_t *>(take(4 * (size_t)nf));
-  uint32_t *l_keys = reinterpret_cast<uint32_t *>(take(4 * (size_t)nf));
-  uint32_t *l_ids_tmp = l_flags, *l_keys_tmp = reinterpret_cast<uint32_t *>(take(4 * (size_t)nf));
-  uint32_t *l_table = reinterpret_cast<uint32_t *>(take(4 * (16 * (size_t)sort_tiles + 1)));
-  uint32_t *l_scratch = reinterpret_cast<uint32_t *>(
-      take(4 * std::max(scan_scratch_words(nf), scan_scratch_words(16 * sort_tiles))));
-  float *l_cdf = reinterpret_cast<float *>(l_offs);  // the offsets are dead once the ids are compacted
-  float *l_total = reinterpret_cast<float *>(take(16));
+  // light table (the sort swaps its key and id buffers)
+  uint32_t *l_ids = m.l_ids, *l_keys = m.l_keys, *l_ids_tmp = m.l_flags, *l_keys_tmp = m.l_keys_tmp;
+  float *l_cdf = reinterpret_cast<float *>(m.l_offs);  // the offsets are dead once the ids are compacted
   sc.cdf = l_cdf;
   sc.light_ids = l_ids;
-  sc.total_area = l_total;
+  sc.total_area = m.l_total;
   sc.n_lights = 0;
 
-  cudaEvent_t e_begin = nullptr, e_end = nullptr;
-  std::vector<cudaEvent_t> ev;
-  struct Events {  // destroyed on every exit
-    std::vector<cudaEvent_t> &v;
-    ~Events() {
-      for (cudaEvent_t e : v)
-        if (e) cudaEventDestroy(e);
-    }
-  } events{ev};
-  if (res) {
-    NRT_CUDA(cudaEventCreate(&e_begin));
-    ev.push_back(e_begin);
-    NRT_CUDA(cudaEventCreate(&e_end));
-    ev.push_back(e_end);
-    NRT_CUDA(cudaEventRecord(e_begin, s));
-  }
-  Timer timer{ev, res != nullptr};
+  PassClock clock(res != nullptr);
+  if (const int rc = clock.start(s)) return rc;
   uint32_t launches = 0, trav_launches = 0;
   NRT_CUDA(cudaMemsetAsync(info, 0, 2 * sizeof(unsigned long long), s));
   NRT_CUDA(cudaMemsetAsync(totals, 0, 3 * sizeof(unsigned long long), s));
-  if (const int rc = wk.light_candidates(sc, nf, l_flags, l_offs, l_ids, l_keys, l_scratch, info, s)) return rc;
+  if (const int rc = wk.light_candidates(sc, nf, m.l_flags, m.l_offs, l_ids, l_keys, m.l_scratch, info, s)) return rc;
   launches += 2 + scan_launches(nf);
   unsigned long long hinfo[2] = {0, 0};
   NRT_CUDA(cudaMemcpyAsync(hinfo, info, sizeof(hinfo), cudaMemcpyDeviceToHost, s));
@@ -859,36 +834,21 @@ int run_pass(Walk &wk, const nrt_bdpt_params &p, const Layout &L, Scene sc, char
     return NRT_ERR_INVALID;
   }
   sc.n_lights = (uint32_t)hinfo[0];
-  light_total_kernel<<<1, 1, 0, s>>>(l_keys, sc.n_lights, l_total);
+  light_total_kernel<<<1, 1, 0, s>>>(l_keys, sc.n_lights, m.l_total);
   NRT_CUDA(cudaGetLastError());
   // (area, face) order: a stable sort on the area bits of the face-ordered ids (areas are >= 0)
-  if (const int rc = radix_sort_pairs(l_keys, l_ids, l_keys_tmp, l_ids_tmp, sc.n_lights, 0, 32, l_table, l_scratch, s))
+  if (const int rc = radix_sort_pairs(l_keys, l_ids, l_keys_tmp, l_ids_tmp, sc.n_lights, 0, 32, m.l_table, m.l_scratch, s))
     return rc;
   sc.light_ids = l_ids;
-  light_cdf_kernel<<<1, 1, 0, s>>>(l_keys, sc.n_lights, l_total, l_cdf);
+  light_cdf_kernel<<<1, 1, 0, s>>>(l_keys, sc.n_lights, m.l_total, l_cdf);
   NRT_CUDA(cudaGetLastError());
   launches += 2 + 8 * (2 + scan_launches(16 * ((sc.n_lights + kSortTile - 1) / kSortTile)));
 
   // wave scratch
-  PathState *st = reinterpret_cast<PathState *>(take(cap * sizeof(PathState)));
+  PathState *st = m.st;
+  uint32_t *const *queue = m.queue;
   Subpaths sp;
   sp.stride = stride;
-  nrt_bdpt_vertex *w_eye = nullptr, *w_light = nullptr;
-  uint32_t *w_ne = nullptr, *w_nl = nullptr;
-  float *w_rgb = nullptr;
-  if (!out) {
-    w_eye = reinterpret_cast<nrt_bdpt_vertex *>(take(cap * stride * sizeof(nrt_bdpt_vertex)));
-    w_light = reinterpret_cast<nrt_bdpt_vertex *>(take(cap * stride * sizeof(nrt_bdpt_vertex)));
-    w_ne = reinterpret_cast<uint32_t *>(take(cap * 4));
-    w_nl = reinterpret_cast<uint32_t *>(take(cap * 4));
-    w_rgb = reinterpret_cast<float *>(take(cap * 12));
-  }
-  uint32_t *queue[2] = {reinterpret_cast<uint32_t *>(take(cap * 4)), reinterpret_cast<uint32_t *>(take(cap * 4))};
-  uint32_t *cnt = reinterpret_cast<uint32_t *>(take(cap * 4));
-  uint32_t *offs = reinterpret_cast<uint32_t *>(take(cap * 4));
-  float3 *emit = reinterpret_cast<float3 *>(take(cap * 12));
-  Conn *conns = reinterpret_cast<Conn *>(take(cap * mc * sizeof(Conn)));
-  uint32_t *scan_scratch = reinterpret_cast<uint32_t *>(take(scan_scratch_words((uint32_t)cap) * 4));
 
   for (unsigned long long s0 = 0; s0 < total_slots; s0 += cap) {
     const uint32_t count = (uint32_t)std::min<unsigned long long>(cap, total_slots - s0);
@@ -904,13 +864,13 @@ int run_pass(Walk &wk, const nrt_bdpt_params &p, const Layout &L, Scene sc, char
       sp.n_eye = out->n_eye + s0;
       sp.n_light = out->n_light + s0;
     } else {
-      sp.eye = w_eye;
-      sp.light = w_light;
-      sp.n_eye = w_ne;
-      sp.n_light = w_nl;
+      sp.eye = m.w_eye;
+      sp.light = m.w_light;
+      sp.n_eye = m.w_ne;
+      sp.n_light = m.w_nl;
     }
     wk.wave(s0);
-    float *rgb = out ? out->rgb + 3 * s0 : w_rgb;
+    float *rgb = out ? out->rgb + 3 * s0 : m.w_rgb;
     const unsigned g = (count + 255) / 256;
     for (int eye = 1; eye >= 0; eye--) {
       NRT_CUDA(cudaMemsetAsync(ctr, 0, 2 * sizeof(unsigned long long), s));
@@ -926,23 +886,23 @@ int run_pass(Walk &wk, const nrt_bdpt_params &p, const Layout &L, Scene sc, char
         NRT_CUDA(cudaGetLastError());
         launches++;
         bool empty = false;
-        if (const int rc = wk.bounce(sc, sp, st, queue[in], queue[in ^ 1], ctr, count, B, eye, timer, launches,
+        if (const int rc = wk.bounce(sc, sp, st, queue[in], queue[in ^ 1], ctr, count, B, eye, clock, launches,
                                      trav_launches, &empty, s))
           return rc;
         if (empty) break;
         in ^= 1;
       }
     }
-    conn_count_kernel<<<(count + 127) / 128, 128, 0, s>>>(sc, B, count, sp, cnt);
+    conn_count_kernel<<<(count + 127) / 128, 128, 0, s>>>(sc, B, count, sp, m.cnt);
     NRT_CUDA(cudaGetLastError());
-    if (const int rc = exclusive_scan_u32_async(cnt, offs, count, scan_scratch, s)) return rc;
-    conn_write_kernel<<<(count + 127) / 128, 128, 0, s>>>(sc, B, count, sp, cnt, offs, conns, emit, ctr + 1);
+    if (const int rc = exclusive_scan_u32_async(m.cnt, m.offs, count, m.scan_scratch, s)) return rc;
+    conn_write_kernel<<<(count + 127) / 128, 128, 0, s>>>(sc, B, count, sp, m.cnt, m.offs, m.conns, m.emit, ctr + 1);
     NRT_CUDA(cudaGetLastError());
     begin_launch_kernel<<<1, 1, 0, s>>>(ctr, totals + 2);
     NRT_CUDA(cudaGetLastError());
     launches += 3 + scan_launches(count);
-    if (const int rc = wk.connect(conns, sp, ctr, (size_t)count * mc, timer, launches, trav_launches, s)) return rc;
-    sample_sum_kernel<<<g, 256, 0, s>>>(count, sp, cnt, offs, conns, emit, rgb);
+    if (const int rc = wk.connect(m.conns, sp, ctr, (size_t)count * mc, clock, launches, trav_launches, s)) return rc;
+    sample_sum_kernel<<<g, 256, 0, s>>>(count, sp, m.cnt, m.offs, m.conns, m.emit, rgb);
     NRT_CUDA(cudaGetLastError());
     launches++;
     if (!out) {
@@ -953,20 +913,15 @@ int run_pass(Walk &wk, const nrt_bdpt_params &p, const Layout &L, Scene sc, char
   }
   if (res) {
     unsigned long long ht[3] = {0, 0, 0};
-    NRT_CUDA(cudaEventRecord(e_end, s));
+    if (const int rc = clock.stop(s)) return rc;
     NRT_CUDA(cudaMemcpyAsync(ht, totals, sizeof(ht), cudaMemcpyDeviceToHost, s));
     NRT_CUDA(cudaStreamSynchronize(s));
-    float tms = 0.0f, total_ms = 0.0f;
-    for (size_t i = 2; i + 1 < ev.size(); i += 2) {
-      float m = 0.0f;
-      NRT_CUDA(cudaEventElapsedTime(&m, ev[i], ev[i + 1]));
-      tms += m;
-    }
-    NRT_CUDA(cudaEventElapsedTime(&total_ms, e_begin, e_end));
+    float total_ms = 0.0f, span[2];
+    if (const int rc = clock.read(&total_ms, span)) return rc;
     res->eye_rays = ht[0];
     res->light_rays = ht[1];
     res->connection_rays = ht[2];
-    res->traverse_ms = tms;
+    res->traverse_ms = span[0];
     res->total_ms = total_ms;
     res->launches = launches;
     res->traverse_launches = trav_launches;
@@ -987,8 +942,8 @@ int run_bdpt(const nrt_accel *h, const nrt_bdpt_params *pp, float *d_accum, cons
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (const int rc = wait_previous_pass(a, s)) return rc;
   const RecordOnExit pass_done{a->pass_done, s};
-  if (const int rc = grow_wave(a, L.light_bytes + L.wave_bytes)) return rc;
-  unsigned long long *c = reinterpret_cast<unsigned long long *>(a->d_counters);
+  Scratch m;
+  if (const int rc = carve_pass_scratch(a, [&](Carver &c) { m = carve_scratch(c, L); })) return rc;
   Scene sc;
   sc.mats = static_cast<const PathMaterial *>(p.d_materials);
   sc.mat_ids = static_cast<const uint32_t *>(p.d_material_ids);
@@ -998,7 +953,8 @@ int run_bdpt(const nrt_accel *h, const nrt_bdpt_params *pp, float *d_accum, cons
   sc.n_materials = p.n_materials;
   FlatWalk wk{a, p.flags};
   // d_counters: [2, 3] lights, bad id; [48, 49] queue counts; [52..54] ray totals
-  return run_pass(wk, p, L, sc, static_cast<char *>(a->d_wave), c + 2, c + 48, c + 52, d_accum, out, res, s, who);
+  return run_pass(wk, p, L, sc, m, pass_counters(a, kWaveCounters), pass_counters(a, kPathCounters),
+                  pass_counters(a, kPathTotals), d_accum, out, res, s, who);
 }
 
 // ---- the scene pass
@@ -1043,7 +999,7 @@ struct SceneWalk {
     return NRT_OK;
   }
   int bounce(const Scene &sc, const Subpaths &sp, PathState *st, const uint32_t *q_in, uint32_t *q_out,
-             unsigned long long *ctr, uint32_t, uint32_t B, int eye, Timer &tm, uint32_t &launches,
+             unsigned long long *ctr, uint32_t, uint32_t B, int eye, PassClock &tm, uint32_t &launches,
              uint32_t &trav_launches, bool *empty, cudaStream_t s) {
     uint32_t n = 0;
     if (const int rc = read_count(ctr, n, s)) return rc;
@@ -1062,7 +1018,7 @@ struct SceneWalk {
     trav_launches++;
     return NRT_OK;
   }
-  int connect(Conn *conns, const Subpaths &sp, unsigned long long *ctr, size_t, Timer &tm, uint32_t &launches,
+  int connect(Conn *conns, const Subpaths &sp, unsigned long long *ctr, size_t, PassClock &tm, uint32_t &launches,
               uint32_t &trav_launches, cudaStream_t s) {
     uint32_t n = 0;
     if (const int rc = read_count(ctr, n, s)) return rc;
@@ -1081,38 +1037,24 @@ struct SceneWalk {
   }
 };
 
-// The device memory of one scene call, released when the call returns
-struct CallBuffer {
-  char *d = nullptr;
-  cudaStream_t s = nullptr;
-  ~CallBuffer() {
-    if (!d) return;
-    cudaStreamSynchronize(s);  // nothing of the call may still use it
-    cudaFree(d);
-  }
-};
-
 int run_scene_bdpt(const nrt_scene *scn, const nrt_bdpt_params *pp, const nrt_scene_shading *shading, float *d_accum,
                    const Out *out, nrt_bdpt_result *res, void *stream, const char *who) {
-  auto bad = [&](const std::string &why) {
-    set_error(std::string(who) + ": " + why);
-    return NRT_ERR_INVALID;
-  };
-  if (!scn || !pp) return bad("NULL argument");
-  if (!shading) return bad("NULL shading array (one nrt_scene_shading per instance)");
+  if (!scn || !pp) return refuse(who, "NULL argument");
+  if (!shading) return refuse(who, "NULL shading array (one nrt_scene_shading per instance)");
   const nrt_bdpt_params p = *pp;
-  if (!p.d_materials || p.n_materials == 0) return bad("materials are required");
+  if (!p.d_materials || p.n_materials == 0) return refuse(who, "materials are required");
   if (p.d_material_ids || p.d_facevarying_normals)
-    return bad("material ids and face-varying normals are given per instance (nrt_scene_shading), not in the params");
+    return refuse(who,
+                  "material ids and face-varying normals are given per instance (nrt_scene_shading), not in the params");
   if (const int rc = check_common(p, who)) return rc;
   const SceneView view = scene_view(scn);
   std::vector<uint32_t> face_offs(view.n + 1, 0u);
   for (uint32_t i = 0; i < view.n; i++) {
-    if (view.n_faces[i] == 0) return bad("triangle instances only");
+    if (view.n_faces[i] == 0) return refuse(who, "triangle instances only");
     if (!shading[i].d_material_ids || !shading[i].d_facevarying_normals)
-      return bad("instance " + std::to_string(i) + " has no material ids or face-varying normals");
+      return refuse(who, "instance " + std::to_string(i) + " has no material ids or face-varying normals");
     const uint64_t next = (uint64_t)face_offs[i] + view.n_faces[i];
-    if (next > 0xFFFFFFFFull) return bad("more than 2^32 - 1 {instance, face} pairs");
+    if (next > 0xFFFFFFFFull) return refuse(who, "more than 2^32 - 1 {instance, face} pairs");
     face_offs[i + 1] = (uint32_t)next;
   }
   const uint32_t n_pairs = face_offs[view.n];
@@ -1121,39 +1063,35 @@ int run_scene_bdpt(const nrt_scene *scn, const nrt_bdpt_params *pp, const nrt_sc
   const size_t extra = (out ? 0 : 2 * (size_t)(p.max_bounces + 1) * 4 + 8) + (size_t)max_conns(p.max_bounces) * per_conn;
   if (const int rc = make_layout(p, out != nullptr, n_pairs, extra, who, L)) return rc;
   const size_t n_rec = (size_t)L.cap * L.mc;
-  const size_t walk_bytes = rnd256(n_rec * sizeof(Ray36)) + rnd256(n_rec * sizeof(SceneHit32)) + rnd256(n_rec) +
-                            (out ? 0 : 2 * rnd256(L.cap * L.stride * 4) + rnd256(L.cap * 8));
-  const size_t table_bytes = rnd256(sizeof(SceneShadingDev) * view.n) + rnd256(4 * ((size_t)view.n + 1)) + rnd256(64);
 
   NRT_DEVICE(view.device);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  CallBuffer buf;
-  buf.s = s;
-  NRT_CUDA(cudaMalloc(&buf.d, L.light_bytes + L.wave_bytes + walk_bytes + table_bytes));
-  char *b = buf.d;
-  char *w = b + L.light_bytes + L.wave_bytes;  // run_pass carves [b, w)
-  auto take = [&](size_t bytes) {
-    char *r = w;
-    w += rnd256(bytes);
-    return r;
-  };
   SceneWalk wk;
   wk.scene = scn;
   wk.flags = p.flags;
   wk.stride = L.stride;
   wk.out = out;
-  wk.rays = reinterpret_cast<Ray36 *>(take(n_rec * sizeof(Ray36)));
-  wk.hits = reinterpret_cast<SceneHit32 *>(take(n_rec * sizeof(SceneHit32)));
-  wk.mask = reinterpret_cast<uint8_t *>(take(n_rec));
   wk.w_sv = SceneVerts{nullptr, nullptr, nullptr};
-  if (!out) {
-    wk.w_sv.eye_inst = reinterpret_cast<uint32_t *>(take(L.cap * L.stride * 4));
-    wk.w_sv.light_inst = reinterpret_cast<uint32_t *>(take(L.cap * L.stride * 4));
-    wk.w_sv.light_pair = reinterpret_cast<uint32_t *>(take(L.cap * 8));
-  }
-  SceneShadingDev *d_shading = reinterpret_cast<SceneShadingDev *>(take(sizeof(SceneShadingDev) * view.n));
-  uint32_t *d_offs = reinterpret_cast<uint32_t *>(take(4 * ((size_t)view.n + 1)));
-  unsigned long long *c = reinterpret_cast<unsigned long long *>(take(64));
+  Scratch m;
+  SceneShadingDev *d_shading = nullptr;
+  uint32_t *d_offs = nullptr;
+  unsigned long long *c = nullptr;
+  CallMemory mem(s);
+  if (const int rc = mem.alloc([&](Carver &k) {
+        m = carve_scratch(k, L);
+        wk.rays = k.take<Ray36>(n_rec);
+        wk.hits = k.take<SceneHit32>(n_rec);
+        wk.mask = k.take<uint8_t>(n_rec);
+        if (!out) {
+          wk.w_sv.eye_inst = k.take<uint32_t>(L.cap * L.stride);
+          wk.w_sv.light_inst = k.take<uint32_t>(L.cap * L.stride);
+          wk.w_sv.light_pair = k.take<uint32_t>(2 * L.cap);
+        }
+        d_shading = k.take<SceneShadingDev>(view.n);
+        d_offs = k.take<uint32_t>((size_t)view.n + 1);
+        c = k.take<unsigned long long>(8);
+      }))
+    return rc;
   NRT_CUDA(cudaMemcpyAsync(d_shading, shading, sizeof(SceneShadingDev) * view.n, cudaMemcpyHostToDevice, s));
   NRT_CUDA(cudaMemcpyAsync(d_offs, face_offs.data(), 4 * face_offs.size(), cudaMemcpyHostToDevice, s));
   wk.g = SceneGeo{static_cast<const InstanceDev *>(view.inst), view.state76, d_shading, d_offs, view.n};
@@ -1161,7 +1099,8 @@ int run_scene_bdpt(const nrt_scene *scn, const nrt_bdpt_params *pp, const nrt_sc
   sc.mats = static_cast<const PathMaterial *>(p.d_materials);
   sc.n_materials = p.n_materials;
   // c: [0, 1] lights, bad id; [2, 3] queue counts; [4..6] ray totals
-  return run_pass(wk, p, L, sc, b, c, c + 2, c + 4, d_accum, out, res, s, who);
+  if (const int rc = run_pass(wk, p, L, sc, m, c, c + 2, c + 4, d_accum, out, res, s, who)) return rc;
+  return mem.drain();
 }
 
 }  // namespace

@@ -242,6 +242,15 @@ struct Accel {
   mutable LaunchRing<32> ring;
 };
 
+// The regions of Accel::d_counters the passes keep their counters in (pass scratch, like d_wave)
+constexpr int kWaveCounters = 2;   // [2, 4): a wave's or a compaction's counters
+constexpr int kPassTotals = 4;     // [4, 7): the AO passes' totals
+constexpr int kPathCounters = 48;  // [48, 52): the path queues' counters
+constexpr int kPathTotals = 52;    // [52, 55): the path tracers' totals
+inline unsigned long long *pass_counters(const Accel *a, int region) {
+  return reinterpret_cast<unsigned long long *>(a->d_counters) + region;
+}
+
 // Passes on one accel (AO passes, path passes, path bounces) share its pass scratch.  Under host_mu, a pass calls
 // wait_previous_pass before it enqueues anything and holds a RecordOnExit for as long as it enqueues, so that every
 // pass runs on the device after the one enqueued before it, whatever streams the two are on.

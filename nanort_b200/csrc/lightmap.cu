@@ -12,6 +12,7 @@
 #include "common.cuh"
 #include "scan.cuh"
 #include "wavefront.cuh"
+#include "pass_host.cuh"
 
 namespace nrt {
 
@@ -83,13 +84,7 @@ int lightmap_check(const Accel *a, const void *d_records, const nrt_lightmap_par
     set_error(std::string(who) + ": NULL argument");
     return NRT_ERR_INVALID;
   }
-  const uint64_t n = (uint64_t)p->width * p->height;
-  if (n == 0 || n > kMaxTexels || p->spp == 0 || p->max_bounces == 0 || p->n_materials == 0 || !p->d_materials ||
-      (p->n_emissive > 0 && !p->d_emissive_faces)) {
-    set_error(std::string(who) + ": width * height must lie in [1, 2^31], spp, max_bounces and n_materials must be "
-                                 "positive, and the materials and emissive faces given");
-    return NRT_ERR_INVALID;
-  }
+  if (const int rc = check_lightmap_params(*p, who)) return rc;
   if (p->flags & ~(uint32_t)(NRT_TRAVERSE_ANY_HIT | NRT_TRAVERSE_CPP03_INVERSE)) {
     set_error(std::string(who) + ": flags other than NRT_TRAVERSE_ANY_HIT / NRT_TRAVERSE_CPP03_INVERSE");
     return NRT_ERR_INVALID;
@@ -104,9 +99,6 @@ int lightmap_check(const Accel *a, const void *d_records, const nrt_lightmap_par
   }
   return NRT_OK;
 }
-
-// scratch of a bake: the compaction's words (bake_prepare), then the queues from a 256-byte boundary
-size_t compaction_bytes(uint32_t n) { return ((2 * (size_t)n + scan_scratch_words(n)) * sizeof(uint32_t) + 255) & ~(size_t)255; }
 
 }  // namespace
 }  // namespace nrt
@@ -131,61 +123,31 @@ extern "C" int nrt_bake_lightmap_device(const nrt_accel *world, const void *d_re
   // the paths of one wave: at most 8 Mi, as in the path pass
   const unsigned long long kMaxWave = 8ull << 20;
   const unsigned long long cap_max = std::min<unsigned long long>(kMaxWave, (unsigned long long)n * lp.spp);
-  // per path: 2 radiance queues (32 + 4 B each), shadow queue (48 B), weight (16 B)
-  const size_t per_path = 2 * (2 * sizeof(float4) + 4) + 3 * sizeof(float4) + sizeof(float4);
-  const size_t lead = compaction_bytes(n);
-  if (const int rc = grow_wave(a, lead + (size_t)cap_max * per_path + 256)) return rc;
+  // the compaction's scratch (bake_prepare), then the queues
+  PathQueues q;
+  const auto scratch = [&](Carver &c, unsigned long long cap) {
+    carve_compaction(c, n);
+    q = carve_path_queues(c, cap);
+  };
+  if (const int rc = carve_pass_scratch(a, [&](Carver &c) { scratch(c, cap_max); })) return rc;
   uint32_t launches = a->d_face_n ? 0u : 1u;
   if (const int rc = ensure_face_normals(a, s)) return rc;
 
-  std::vector<cudaEvent_t> ev;
-  struct Events {  // destroyed on every exit
-    std::vector<cudaEvent_t> &v;
-    ~Events() {
-      for (cudaEvent_t e : v)
-        if (e) cudaEventDestroy(e);
-    }
-  } events{ev};
-  auto record = [&]() -> int {
-    cudaEvent_t e = nullptr;
-    NRT_CUDA(cudaEventCreate(&e));
-    ev.push_back(e);
-    NRT_CUDA(cudaEventRecord(e, s));
-    return NRT_OK;
-  };
-  if (res) {
-    if (const int rc = record()) return rc;  // ev[0]: begin
-  }
+  PassClock clock(res != nullptr);
+  if (const int rc = clock.start(s)) return rc;
   uint32_t *list = nullptr, n_cov = 0;
   if (const int rc = bake_prepare(a, d_records_16B, n, who, s, &list, &n_cov, &launches)) return rc;
   const unsigned long long total = (unsigned long long)n_cov * lp.spp;
   const unsigned long long cap = std::min(total, kMaxWave);
-  PathQueues q;
-  {
-    char *b = static_cast<char *>(a->d_wave) + lead;
-    auto take = [&](size_t bytes) {
-      char *r = b;
-      b += bytes;
-      return r;
-    };
-    for (int k = 0; k < 2; k++) {
-      q.org_tmin[k] = reinterpret_cast<float4 *>(take(cap * sizeof(float4)));
-      q.dir_tmax[k] = reinterpret_cast<float4 *>(take(cap * sizeof(float4)));
-    }
-    q.sh_org_tmin = reinterpret_cast<float4 *>(take(cap * sizeof(float4)));
-    q.sh_dir_tmax = reinterpret_cast<float4 *>(take(cap * sizeof(float4)));
-    q.sh_contrib_pix = reinterpret_cast<float4 *>(take(cap * sizeof(float4)));
-    q.weight = reinterpret_cast<float4 *>(take(cap * sizeof(float4)));
-    for (int k = 0; k < 2; k++) q.path_id[k] = reinterpret_cast<uint32_t *>(take(cap * 4));
-  }
-  unsigned long long *ctr = reinterpret_cast<unsigned long long *>(a->d_counters) + 48;     // [48..51]
-  unsigned long long *totals = reinterpret_cast<unsigned long long *>(a->d_counters) + 52;  // [52..53]
+  Carver c(a->d_wave);
+  scratch(c, cap);
+  unsigned long long *ctr = pass_counters(a, kPathCounters);   // [48..51]
+  unsigned long long *totals = pass_counters(a, kPathTotals);  // [52..53]
   NRT_CUDA(cudaMemsetAsync(ctr, 0, 6 * sizeof(unsigned long long), s));
   const TraceOptions16 opt = default_trace_options();
   const float4 *records = static_cast<const float4 *>(d_records_16B);
   const FastDiv n_cov_div(n_cov);
   uint32_t trav_launches = 0;
-  std::vector<std::pair<size_t, size_t>> trav_ev;  // (start, end) event indices around traversal launches
   for (unsigned long long s0 = 0; s0 < total; s0 += cap) {
     const uint32_t count = (uint32_t)std::min(cap, total - s0);
     const TexelSlots slots{list, n_cov_div, (uint32_t)(s0 % n_cov), (uint32_t)(s0 / n_cov)};
@@ -195,10 +157,7 @@ extern "C" int nrt_bake_lightmap_device(const nrt_accel *world, const void *d_re
     NRT_CUDA(cudaGetLastError());
     launches++;
     for (uint32_t b = 0; b < lp.max_bounces; b++) {
-      const size_t e0 = ev.size();
-      if (res) {
-        if (const int rc = record()) return rc;
-      }
+      if (const int rc = clock.begin(s)) return rc;
       if (b > 0) {
         const LightmapShadeEpilogue epi{p, slots, (int)(b & 1u), b, q, a->d_verts, a->d_faces, d_accum_rgb, ctr};
         if (const int rc = launch_traverse_lightmap_radiance(a, epi, ctr + 3, count, opt, lp.flags, s)) return rc;
@@ -208,32 +167,24 @@ extern "C" int nrt_bake_lightmap_device(const nrt_accel *world, const void *d_re
       if (const int rc = launch_traverse_path_shadow(a, q, ctr + 1, count, d_accum_rgb, opt, lp.flags, s)) return rc;
       launches++;
       trav_launches++;
-      if (res) {
-        if (const int rc = record()) return rc;
-        trav_ev.emplace_back(e0, ev.size() - 1);
-      }
+      if (const int rc = clock.end(s)) return rc;
       next_bounce_kernel<<<1, 1, 0, s>>>(ctr, totals);
       NRT_CUDA(cudaGetLastError());
       launches++;
     }
   }
   if (res) {
-    if (const int rc = record()) return rc;  // end
+    if (const int rc = clock.stop(s)) return rc;
     unsigned long long ht[2] = {0, 0};
     NRT_CUDA(cudaMemcpyAsync(ht, totals, sizeof(ht), cudaMemcpyDeviceToHost, s));
     NRT_CUDA(cudaStreamSynchronize(s));
-    float tms = 0.0f, total_ms = 0.0f;
-    for (const auto &se : trav_ev) {
-      float m = 0.0f;
-      NRT_CUDA(cudaEventElapsedTime(&m, ev[se.first], ev[se.second]));
-      tms += m;
-    }
-    NRT_CUDA(cudaEventElapsedTime(&total_ms, ev.front(), ev.back()));
+    float total_ms = 0.0f, span[2];
+    if (const int rc = clock.read(&total_ms, span)) return rc;
     res->texels = n_cov;
     res->paths = total;
     res->radiance_rays = ht[0];
     res->shadow_rays = ht[1];
-    res->traverse_ms = tms;
+    res->traverse_ms = span[0];
     res->total_ms = total_ms;
     res->launches = launches;
     res->traverse_launches = trav_launches;
@@ -273,7 +224,7 @@ extern "C" int nrt_bake_lightmap_bounce_device(const nrt_accel *world, const voi
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (const int rc = wait_previous_pass(a, s)) return rc;
   const RecordOnExit pass_done{a->pass_done, s};
-  if (const int rc = grow_wave(a, compaction_bytes(n))) return rc;
+  if (const int rc = carve_pass_scratch(a, [&](Carver &c) { carve_compaction(c, n); })) return rc;
   if (const int rc = ensure_face_normals(a, s)) return rc;
   uint32_t *list = nullptr, n_cov = 0, launches = 0;
   if (const int rc = bake_prepare(a, d_records_16B, n, who, s, &list, &n_cov, &launches)) return rc;
@@ -285,18 +236,9 @@ extern "C" int nrt_bake_lightmap_bounce_device(const nrt_accel *world, const voi
     set_error(std::string(who) + ": the records cover no texel");
     return NRT_ERR_INVALID;
   }
-  PathQueues q;
-  q.org_tmin[0] = static_cast<float4 *>(const_cast<void *>(d_org_tmin));
-  q.dir_tmax[0] = static_cast<float4 *>(const_cast<void *>(d_dir_tmax));
-  q.path_id[0] = const_cast<uint32_t *>(d_path_id);
-  q.org_tmin[1] = static_cast<float4 *>(d_out_org_tmin);
-  q.dir_tmax[1] = static_cast<float4 *>(d_out_dir_tmax);
-  q.path_id[1] = d_out_path_id;
-  q.sh_org_tmin = static_cast<float4 *>(d_sh_org_tmin);
-  q.sh_dir_tmax = static_cast<float4 *>(d_sh_dir_tmax);
-  q.sh_contrib_pix = static_cast<float4 *>(d_sh_contrib_pix);
-  q.weight = static_cast<float4 *>(d_weight);
-  unsigned long long *ctr = reinterpret_cast<unsigned long long *>(a->d_counters) + 48;  // [0] cont, [1] shadow, [3] n
+  const PathQueues q = caller_path_queues(d_org_tmin, d_dir_tmax, d_path_id, d_weight, d_out_org_tmin, d_out_dir_tmax,
+                                         d_out_path_id, d_sh_org_tmin, d_sh_dir_tmax, d_sh_contrib_pix);
+  unsigned long long *ctr = pass_counters(a, kPathCounters);  // [0] cont, [1] shadow, [3] n
   const unsigned long long init[4] = {0ull, 0ull, 0ull, (unsigned long long)n_rays};
   NRT_CUDA(cudaMemcpyAsync(ctr, init, sizeof(init), cudaMemcpyHostToDevice, s));
   const TraceOptions16 opt = default_trace_options();
@@ -314,10 +256,6 @@ extern "C" int nrt_bake_lightmap_bounce_device(const nrt_accel *world, const voi
     if (const int rc = launch_traverse_path_shadow(a, q, ctr + 1, (size_t)n_rays, d_accum_rgb, opt, lp.flags, s))
       return rc;
   }
-  unsigned long long out[2] = {0, 0};
-  NRT_CUDA(cudaMemcpyAsync(out, ctr, sizeof(out), cudaMemcpyDeviceToHost, s));
-  NRT_CUDA(cudaStreamSynchronize(s));
-  if (n_continue) *n_continue = out[0];
-  if (n_shadow) *n_shadow = out[1];
-  return NRT_OK;
+  unsigned long long counts[2] = {0, 0};
+  return finish_bounce(ctr, counts, n_continue, n_shadow, s);
 }

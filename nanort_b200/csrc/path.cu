@@ -9,6 +9,7 @@
 
 #include "common.cuh"
 #include "wavefront.cuh"
+#include "pass_host.cuh"
 
 namespace nrt {
 
@@ -91,12 +92,7 @@ extern "C" int nrt_render_path_device(const nrt_accel *h, const nrt_path_params 
   }
   Accel *a = const_cast<Accel *>(reinterpret_cast<const Accel *>(h));
   const nrt_path_params p = *pp;
-  if (p.width == 0 || p.height == 0 || p.spp == 0 || p.n_shards == 0 || p.shard >= p.n_shards || p.tile_w == 0 ||
-      p.tile_h == 0 || (p.tile_w % 8) != 0 || (p.tile_h % 4) != 0 || p.max_bounces == 0 || p.n_materials == 0 ||
-      !p.d_materials || (p.n_emissive > 0 && !p.d_emissive_faces)) {
-    set_error("nrt_render_path_device: bad parameters");
-    return NRT_ERR_INVALID;
-  }
+  if (const int rc = check_path_params(p, "nrt_render_path_device")) return rc;
   NRT_DEVICE(a->device);
   // d_wave / d_counters[48..54] are per-accel scratch, shared with AO passes and path bounces: the pass waits on the
   // device for the previous pass on this accel (render.cu)
@@ -104,111 +100,57 @@ extern "C" int nrt_render_path_device(const nrt_accel *h, const nrt_path_params 
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (const int rc = wait_previous_pass(a, s)) return rc;
   const RecordOnExit pass_done{a->pass_done, s};
-  const uint32_t tiles_x = (p.width + p.tile_w - 1) / p.tile_w, tiles_y = (p.height + p.tile_h - 1) / p.tile_h;
-  const uint32_t n_tiles = tiles_x * tiles_y;
-  const uint32_t my_tiles = n_tiles > p.shard ? (n_tiles - p.shard + p.n_shards - 1) / p.n_shards : 0;
-  const unsigned long long per_tile = (unsigned long long)p.tile_w * p.tile_h * p.spp;
-  const unsigned long long total_slots = (unsigned long long)my_tiles * per_tile;
-  const unsigned long long kMaxWave = 8ull << 20;
-  unsigned long long tiles_per_wave = kMaxWave / per_tile;
-  if (tiles_per_wave == 0) tiles_per_wave = 1;
-  const unsigned long long cap = std::min<unsigned long long>(total_slots, tiles_per_wave * per_tile);
-  // per path: 2 radiance queues (32 + 4 B each), shadow queue (48 B), weight (16 B)
-  const size_t per_path = 2 * (2 * sizeof(float4) + 4) + 3 * sizeof(float4) + sizeof(float4);
-  const size_t need = (size_t)cap * per_path + 256;
-  if (const int rc = grow_wave(a, need)) return rc;
+  const ShardSlots sh = shard_slots(p.width, p.height, p.tile_w, p.tile_h, p.spp, p.shard, p.n_shards);
+  const unsigned long long total_slots = sh.total;
+  const unsigned long long cap = sh.wave(8ull << 20);
   PathQueues q;
-  {
-    char *b = static_cast<char *>(a->d_wave);
-    auto take = [&](size_t bytes) {
-      char *r = b;
-      b += bytes;
-      return r;
-    };
-    for (int k = 0; k < 2; k++) {
-      q.org_tmin[k] = reinterpret_cast<float4 *>(take(cap * sizeof(float4)));
-      q.dir_tmax[k] = reinterpret_cast<float4 *>(take(cap * sizeof(float4)));
-    }
-    q.sh_org_tmin = reinterpret_cast<float4 *>(take(cap * sizeof(float4)));
-    q.sh_dir_tmax = reinterpret_cast<float4 *>(take(cap * sizeof(float4)));
-    q.sh_contrib_pix = reinterpret_cast<float4 *>(take(cap * sizeof(float4)));
-    q.weight = reinterpret_cast<float4 *>(take(cap * sizeof(float4)));
-    for (int k = 0; k < 2; k++) q.path_id[k] = reinterpret_cast<uint32_t *>(take(cap * 4));
-  }
-  unsigned long long *ctr = reinterpret_cast<unsigned long long *>(a->d_counters) + 48;     // [48..51]
-  unsigned long long *totals = reinterpret_cast<unsigned long long *>(a->d_counters) + 52;  // [52..54]
+  if (const int rc = carve_pass_scratch(a, [&](Carver &c) { q = carve_path_queues(c, cap); })) return rc;
+  unsigned long long *ctr = pass_counters(a, kPathCounters);   // [48..51]
+  unsigned long long *totals = pass_counters(a, kPathTotals);  // [52..54]
   NRT_CUDA(cudaMemsetAsync(ctr, 0, 8 * sizeof(unsigned long long), s));
 
   const TraceOptions16 opt = default_trace_options();
   const uint32_t trav_flags = p.flags & 0xFFFFu;
-  cudaEvent_t e_begin = nullptr, e_end = nullptr;
-  std::vector<cudaEvent_t> ev;
-  if (res) {
-    NRT_CUDA(cudaEventCreate(&e_begin));
-    NRT_CUDA(cudaEventCreate(&e_end));
-    NRT_CUDA(cudaEventRecord(e_begin, s));
-  }
+  PassClock clock(res != nullptr);
+  if (const int rc = clock.start(s)) return rc;
   uint32_t launches = 0, trav_launches = 0;
-  int rc = NRT_OK;
-  for (unsigned long long s0 = 0; s0 < total_slots && rc == NRT_OK; s0 += cap) {
+  for (unsigned long long s0 = 0; s0 < total_slots; s0 += cap) {
     const uint32_t count = (uint32_t)std::min<unsigned long long>(cap, total_slots - s0);
-    cudaMemsetAsync(ctr, 0, 4 * sizeof(unsigned long long), s);
+    NRT_CUDA(cudaMemsetAsync(ctr, 0, 4 * sizeof(unsigned long long), s));
     gen_camera_kernel<<<(count + 255) / 256, 256, 0, s>>>(p, s0, count, q, ctr);
     launches++;
     int in = 0;
-    for (uint32_t b = 0; b < p.max_bounces && rc == NRT_OK; b++) {
+    for (uint32_t b = 0; b < p.max_bounces; b++) {
       begin_bounce_kernel<<<1, 1, 0, s>>>(ctr, totals, count, b == 0 ? 1 : 0);
-      cudaEvent_t t0 = nullptr, t1 = nullptr;
-      if (res) {
-        cudaEventCreate(&t0);
-        cudaEventCreate(&t1);
-        ev.push_back(t0);
-        ev.push_back(t1);
-        cudaEventRecord(t0, s);
-      }
+      if (const int rc = clock.begin(s)) return rc;
       PathShadeEpilogue epi{p, TileSlots{s0}, in, b, q, a->d_verts, a->d_faces, d_accum_rgb, ctr};
-      rc = launch_traverse_path_radiance(a, epi, ctr + 3, count, opt, trav_flags, s);
-      if (rc != NRT_OK) break;
-      rc = launch_traverse_path_shadow(a, q, ctr + 1, count, d_accum_rgb, opt, trav_flags, s);
-      if (rc != NRT_OK) break;
-      if (res) cudaEventRecord(t1, s);
+      if (const int rc = launch_traverse_path_radiance(a, epi, ctr + 3, count, opt, trav_flags, s)) return rc;
+      if (const int rc = launch_traverse_path_shadow(a, q, ctr + 1, count, d_accum_rgb, opt, trav_flags, s)) return rc;
+      if (const int rc = clock.end(s)) return rc;
       end_bounce_kernel<<<1, 1, 0, s>>>(ctr, totals);
       launches += 4;
       trav_launches += 2;
       in ^= 1;
     }
-    if (cudaGetLastError() != cudaSuccess) rc = NRT_ERR_CUDA;
+    NRT_CUDA(cudaGetLastError());
   }
-  if (rc == NRT_OK && res) {
+  if (res) {
     unsigned long long ht[3] = {0, 0, 0};
-    cudaEventRecord(e_end, s);
-    cudaError_t e = cudaMemcpyAsync(ht, totals, sizeof(ht), cudaMemcpyDeviceToHost, s);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess) {
-      rc = cuda_fail(e, "nrt_render_path_device read-back", __FILE__, __LINE__);
-    } else {
-      res->radiance_rays = ht[0];
-      res->shadow_rays = ht[1];
-      res->camera_rays = ht[2];
-      float tms = 0.0f, total = 0.0f;
-      for (size_t i = 0; i + 1 < ev.size(); i += 2) {
-        float m1 = 0;
-        cudaEventElapsedTime(&m1, ev[i], ev[i + 1]);
-        tms += m1;
-      }
-      cudaEventElapsedTime(&total, e_begin, e_end);
-      res->traverse_ms = tms;
-      res->total_ms = total;
-      res->launches = launches;
-      res->traverse_launches = trav_launches;
-    }
+    if (const int rc = clock.stop(s)) return rc;
+    NRT_CUDA(cudaMemcpyAsync(ht, totals, sizeof(ht), cudaMemcpyDeviceToHost, s));
+    NRT_CUDA(cudaStreamSynchronize(s));
+    float total_ms = 0.0f, span[2];
+    if (const int rc = clock.read(&total_ms, span)) return rc;
+    res->radiance_rays = ht[0];
+    res->shadow_rays = ht[1];
+    res->camera_rays = ht[2];
+    res->traverse_ms = span[0];
+    res->total_ms = total_ms;
+    res->launches = launches;
+    res->traverse_launches = trav_launches;
   }
-  for (cudaEvent_t e : ev) cudaEventDestroy(e);
-  if (e_begin) cudaEventDestroy(e_begin);
-  if (e_end) cudaEventDestroy(e_end);
-  return rc;
+  return NRT_OK;
 }
-
 
 // One bounce of the wavefront path tracer on caller-owned queues: traverses the n radiance rays, runs the reference's
 // per-hit shading block in the retire step (PathShadeEpilogue), appends the continuation rays and the shadow (next-event)
@@ -228,12 +170,7 @@ extern "C" int nrt_path_bounce_device(const nrt_accel *h, const nrt_path_params 
   }
   Accel *a = const_cast<Accel *>(reinterpret_cast<const Accel *>(h));
   const nrt_path_params p = *pp;
-  if (p.width == 0 || p.height == 0 || p.spp == 0 || p.n_shards == 0 || p.shard >= p.n_shards || p.tile_w == 0 ||
-      p.tile_h == 0 || (p.tile_w % 8) != 0 || (p.tile_h % 4) != 0 || p.max_bounces == 0 || p.n_materials == 0 ||
-      !p.d_materials || (p.n_emissive > 0 && !p.d_emissive_faces)) {
-    set_error("nrt_path_bounce_device: bad parameters");
-    return NRT_ERR_INVALID;
-  }
+  if (const int rc = check_path_params(p, "nrt_path_bounce_device")) return rc;
   if (n_continue) *n_continue = 0;
   if (n_shadow) *n_shadow = 0;
   if (n_rays == 0) return NRT_OK;
@@ -243,18 +180,9 @@ extern "C" int nrt_path_bounce_device(const nrt_accel *h, const nrt_path_params 
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (const int rc = wait_previous_pass(a, s)) return rc;
   const RecordOnExit pass_done{a->pass_done, s};
-  PathQueues q;
-  q.org_tmin[0] = static_cast<float4 *>(const_cast<void *>(d_org_tmin));
-  q.dir_tmax[0] = static_cast<float4 *>(const_cast<void *>(d_dir_tmax));
-  q.path_id[0] = const_cast<uint32_t *>(d_path_id);
-  q.org_tmin[1] = static_cast<float4 *>(d_out_org_tmin);
-  q.dir_tmax[1] = static_cast<float4 *>(d_out_dir_tmax);
-  q.path_id[1] = d_out_path_id;
-  q.sh_org_tmin = static_cast<float4 *>(d_sh_org_tmin);
-  q.sh_dir_tmax = static_cast<float4 *>(d_sh_dir_tmax);
-  q.sh_contrib_pix = static_cast<float4 *>(d_sh_contrib_pix);
-  q.weight = static_cast<float4 *>(d_weight);
-  unsigned long long *ctr = reinterpret_cast<unsigned long long *>(a->d_counters) + 48;  // [0] cont, [1] shadow, [3] n
+  const PathQueues q = caller_path_queues(d_org_tmin, d_dir_tmax, d_path_id, d_weight, d_out_org_tmin, d_out_dir_tmax,
+                                         d_out_path_id, d_sh_org_tmin, d_sh_dir_tmax, d_sh_contrib_pix);
+  unsigned long long *ctr = pass_counters(a, kPathCounters);  // [0] cont, [1] shadow, [3] n
   const unsigned long long init[4] = {0ull, 0ull, 0ull, (unsigned long long)n_rays};
   NRT_CUDA(cudaMemcpyAsync(ctr, init, sizeof(init), cudaMemcpyHostToDevice, s));
   const TraceOptions16 opt = default_trace_options();
@@ -266,10 +194,6 @@ extern "C" int nrt_path_bounce_device(const nrt_accel *h, const nrt_path_params 
     rc = launch_traverse_path_shadow(a, q, ctr + 1, (size_t)n_rays, d_accum_rgb, opt, trav_flags, s);
     if (rc != NRT_OK) return rc;
   }
-  unsigned long long out[2] = {0, 0};
-  NRT_CUDA(cudaMemcpyAsync(out, ctr, sizeof(out), cudaMemcpyDeviceToHost, s));
-  NRT_CUDA(cudaStreamSynchronize(s));
-  if (n_continue) *n_continue = out[0];
-  if (n_shadow) *n_shadow = out[1];
-  return NRT_OK;
+  unsigned long long counts[2] = {0, 0};
+  return finish_bounce(ctr, counts, n_continue, n_shadow, s);
 }

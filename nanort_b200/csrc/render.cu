@@ -15,6 +15,7 @@
 
 #include "common.cuh"
 #include "wavefront.cuh"
+#include "pass_host.cuh"
 
 namespace nrt {
 
@@ -202,52 +203,30 @@ static int run_ao_pass(const nrt_accel *h, const nrt_ao_params *pp, float *d_acc
   if (const int rc = wait_previous_pass(a, s)) return rc;
   const RecordOnExit pass_done{a->pass_done, s};
   if (const int rc = ensure_face_normals(a, s)) return rc;
-  const uint32_t tiles_x = (p.width + p.tile_w - 1) / p.tile_w, tiles_y = (p.height + p.tile_h - 1) / p.tile_h;
-  const uint32_t n_tiles = tiles_x * tiles_y;
-  const uint32_t my_tiles = n_tiles > p.shard ? (n_tiles - p.shard + p.n_shards - 1) / p.n_shards : 0;
-  const unsigned long long per_tile = (unsigned long long)p.tile_w * p.tile_h * p.spp;
-  const unsigned long long total_slots = (unsigned long long)my_tiles * per_tile;
-
+  const ShardSlots sh = shard_slots(p.width, p.height, p.tile_w, p.tile_h, p.spp, p.shard, p.n_shards);
+  const unsigned long long total_slots = sh.total;
   // wave capacity: whole tiles, at most 16 Mi camera rays; the compacted AO queue of such a wave (~9 M rays x
   // 36 B = 330 MB) is written by the primary launch and read back by the AO launch -- 6.6 x the 50 MB L2
-  const unsigned long long kMaxWave = 16ull << 20;
-  unsigned long long tiles_per_wave = kMaxWave / per_tile;
-  if (tiles_per_wave == 0) tiles_per_wave = 1;
-  const unsigned long long cap = std::min<unsigned long long>(total_slots, tiles_per_wave * per_tile);
-  const size_t per_ray = 2 * sizeof(float4) + sizeof(Hit16) + 4 + 2 * sizeof(float4) + 4 + sizeof(Hit16);
-  const size_t need = (size_t)cap * per_ray + 256;
-  if (const int rc = grow_wave(a, need)) return rc;
+  const unsigned long long cap = sh.wave(16ull << 20);
   Wave w;
-  {
-    char *b = static_cast<char *>(a->d_wave);
-    w.org_tmin = reinterpret_cast<float4 *>(b);
-    b += cap * sizeof(float4);
-    w.dir_tmax = reinterpret_cast<float4 *>(b);
-    b += cap * sizeof(float4);
-    w.ao_org_tmin = reinterpret_cast<float4 *>(b);
-    b += cap * sizeof(float4);
-    w.ao_dir_tmax = reinterpret_cast<float4 *>(b);
-    b += cap * sizeof(float4);
-    w.hits = reinterpret_cast<Hit16 *>(b);
-    b += cap * sizeof(Hit16);
-    w.ao_hits = reinterpret_cast<Hit16 *>(b);
-    b += cap * sizeof(Hit16);
-    w.pix = reinterpret_cast<uint32_t *>(b);
-    b += cap * 4;
-    w.ao_pix = reinterpret_cast<uint32_t *>(b);
-  }
-  unsigned long long *wave_ctr = reinterpret_cast<unsigned long long *>(a->d_counters) + 2;  // [2],[3]
-  unsigned long long *totals = reinterpret_cast<unsigned long long *>(a->d_counters) + 4;    // [4..6]
+  if (const int rc = carve_pass_scratch(a, [&](Carver &c) {
+        w.org_tmin = c.take<float4>(cap);
+        w.dir_tmax = c.take<float4>(cap);
+        w.ao_org_tmin = c.take<float4>(cap);
+        w.ao_dir_tmax = c.take<float4>(cap);
+        w.hits = c.take<Hit16>(cap);
+        w.ao_hits = c.take<Hit16>(cap);
+        w.pix = c.take<uint32_t>(cap);
+        w.ao_pix = c.take<uint32_t>(cap);
+      }))
+    return rc;
+  unsigned long long *wave_ctr = pass_counters(a, kWaveCounters);  // [2],[3]
+  unsigned long long *totals = pass_counters(a, kPassTotals);      // [4..6]
   NRT_CUDA(cudaMemsetAsync(totals, 0, 3 * sizeof(unsigned long long), s));
 
   TraceOptions16 opt = default_trace_options();
-  std::vector<cudaEvent_t> ev;
-  cudaEvent_t e_begin = nullptr, e_end = nullptr;
-  if (res) {
-    NRT_CUDA(cudaEventCreate(&e_begin));
-    NRT_CUDA(cudaEventCreate(&e_end));
-    NRT_CUDA(cudaEventRecord(e_begin, s));
-  }
+  PassClock clock(res != nullptr);
+  if (const int rc = clock.start(s)) return rc;
   uint32_t launches = 0, trav_launches = 0;
   unsigned long long dumped_ao = 0, valid_primaries_host = 0;
   const bool fused = !dump_primary && !dump_ao && !(p.flags & NRT_AO_UNFUSED);
@@ -268,34 +247,23 @@ static int run_ao_pass(const nrt_accel *h, const nrt_ao_params *pp, float *d_acc
       gen_primary_kernel<<<grid, 256, 0, s>>>(p, s0, count, w, wave_ctr);
       launches++;
     }
-    cudaEvent_t t0 = nullptr, t1 = nullptr, t2 = nullptr, t3 = nullptr;
-    if (res) {
-      cudaError_t ee = cudaEventCreate(&t0);
-      if (ee == cudaSuccess) ee = cudaEventCreate(&t1);
-      if (ee == cudaSuccess) ee = cudaEventCreate(&t2);
-      if (ee == cudaSuccess) ee = cudaEventCreate(&t3);
-      ev.push_back(t0);  // pushed even on failure: the clean-up loop below destroys whatever was created
-      ev.push_back(t1);
-      ev.push_back(t2);
-      ev.push_back(t3);
-      if (ee != cudaSuccess) {
-        rc = cuda_fail(ee, "cudaEventCreate", __FILE__, __LINE__);
-        break;
-      }
-    }
+    // a traversal launch between the clock's marks, tag 0 for camera rays and 1 for AO rays
+    const auto timed = [&](int tag, auto &&launch) -> int {
+      if (const int rc = clock.begin(s)) return rc;
+      if (const int rc = launch()) return rc;
+      return clock.end(s, tag);
+    };
     if (fused) {
       // two traversal launches per wave and nothing else: camera rays are generated at ray fetch, the retire
       // steps spawn the AO rays and accumulate visibility
-      if (res) cudaEventRecord(t0, s);
-      rc = launch_traverse_camera_fused(a, w, p, s0, count, a->d_face_n, d_accum, wave_ctr, opt, trav_flags, s);
-      if (rc != NRT_OK) break;
-      if (res) {
-        cudaEventRecord(t1, s);
-        cudaEventRecord(t2, s);
-      }
-      rc = launch_traverse_ao_fused(a, w, wave_ctr, count, d_accum, totals, opt, trav_flags, s);
-      if (rc != NRT_OK) break;
-      if (res) cudaEventRecord(t3, s);
+      if ((rc = timed(0, [&] {
+             return launch_traverse_camera_fused(a, w, p, s0, count, a->d_face_n, d_accum, wave_ctr, opt, trav_flags, s);
+           })))
+        break;
+      if ((rc = timed(1, [&] {
+             return launch_traverse_ao_fused(a, w, wave_ctr, count, d_accum, totals, opt, trav_flags, s);
+           })))
+        break;
       fold_wave_counters_kernel<<<1, 1, 0, s>>>(wave_ctr, totals);
       launches += 3;
       trav_launches += 2;
@@ -305,10 +273,8 @@ static int run_ao_pass(const nrt_accel *h, const nrt_ao_params *pp, float *d_acc
         soa_to_aos_kernel<<<grid, 256, 0, s>>>(w.org_tmin, w.dir_tmax, nullptr, count, dump_primary + s0, 1u);
         launches++;
       }
-      if (res) cudaEventRecord(t0, s);
-      rc = launch_traverse_soa(a, w.org_tmin, w.dir_tmax, count, w.hits, opt, trav_flags, s);
-      if (rc != NRT_OK) break;
-      if (res) cudaEventRecord(t1, s);
+      if ((rc = timed(0, [&] { return launch_traverse_soa(a, w.org_tmin, w.dir_tmax, count, w.hits, opt, trav_flags, s); })))
+        break;
       launches++;
       trav_launches++;
       gen_ao_kernel<<<grid, 256, 0, s>>>(p, s0, count, w, a->d_face_n, d_accum, wave_ctr);
@@ -321,10 +287,11 @@ static int run_ao_pass(const nrt_accel *h, const nrt_ao_params *pp, float *d_acc
         cudaStreamSynchronize(s);
         dumped_ao += n_wave;
       }
-      if (res) cudaEventRecord(t2, s);
-      rc = launch_traverse_soa_devcount(a, w.ao_org_tmin, w.ao_dir_tmax, wave_ctr, count, w.ao_hits, opt, trav_flags, s);
-      if (rc != NRT_OK) break;
-      if (res) cudaEventRecord(t3, s);
+      if ((rc = timed(1, [&] {
+             return launch_traverse_soa_devcount(a, w.ao_org_tmin, w.ao_dir_tmax, wave_ctr, count, w.ao_hits, opt,
+                                                 trav_flags, s);
+           })))
+        break;
       launches++;
       trav_launches++;
       accumulate_ao_kernel<<<grid, 256, 0, s>>>(w, wave_ctr, d_accum, totals);
@@ -334,40 +301,25 @@ static int run_ao_pass(const nrt_accel *h, const nrt_ao_params *pp, float *d_acc
   }
   if (rc != NRT_OK && cudaGetLastError() != cudaSuccess && std::string(nrt_last_error()).empty())
     set_error("nrt_render_ao_device: CUDA launch failure");
+  if (n_ao_out) *n_ao_out = dumped_ao;
   if (rc == NRT_OK && res) {
     unsigned long long ht[3] = {0, 0, 0};
-    cudaEventRecord(e_end, s);
+    if ((rc = clock.stop(s))) return rc;
     cudaError_t e = cudaMemcpyAsync(ht, totals, sizeof(ht), cudaMemcpyDeviceToHost, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess) {
-      rc = cuda_fail(e, "nrt_render_ao_device read-back", __FILE__, __LINE__);
-    } else {
-      res->ao_rays = ht[0];
-      res->ao_hits = ht[1];
-      res->primary_rays = ht[2] + valid_primaries_host;
-      float tms = 0.0f, total = 0.0f, tp = 0.0f, ta = 0.0f;
-      for (size_t i = 0; i + 3 < ev.size(); i += 4) {
-        float m1 = 0, m2 = 0;
-        cudaEventElapsedTime(&m1, ev[i], ev[i + 1]);
-        cudaEventElapsedTime(&m2, ev[i + 2], ev[i + 3]);
-        tms += m1 + m2;
-        tp += m1;
-        ta += m2;
-      }
-      cudaEventElapsedTime(&total, e_begin, e_end);
-      res->traverse_ms = tms;
-      res->primary_traverse_ms = tp;
-      res->ao_traverse_ms = ta;
-      res->total_ms = total;
-      res->launches = launches;
-      res->traverse_launches = trav_launches;
-    }
+    if (e != cudaSuccess) return cuda_fail(e, "nrt_render_ao_device read-back", __FILE__, __LINE__);
+    float total = 0.0f, span[2];
+    if ((rc = clock.read(&total, span))) return rc;
+    res->ao_rays = ht[0];
+    res->ao_hits = ht[1];
+    res->primary_rays = ht[2] + valid_primaries_host;
+    res->traverse_ms = span[0] + span[1];
+    res->primary_traverse_ms = span[0];
+    res->ao_traverse_ms = span[1];
+    res->total_ms = total;
+    res->launches = launches;
+    res->traverse_launches = trav_launches;
   }
-  for (cudaEvent_t e : ev)
-    if (e) cudaEventDestroy(e);
-  if (e_begin) cudaEventDestroy(e_begin);
-  if (e_end) cudaEventDestroy(e_end);
-  if (n_ao_out) *n_ao_out = dumped_ao;
   return rc;
 }
 

@@ -825,6 +825,7 @@ int nrt_scene_traverse(const nrt_scene *s, const void *rays_36B, size_t n_rays, 
 // ao_min_t along the normal, occluded iff the reported distance is below ao_max_t (see scene_gen_ao_kernel).
 // Stand-alone stage kernels (the scene walk has no retire-step functor); one host read of the AO count per wave.
 #include "wavefront.cuh"
+#include "pass_host.cuh"
 
 namespace nrt {
 namespace {
@@ -939,17 +940,6 @@ __global__ void __launch_bounds__(256)
   if ((threadIdx.x & 31) == 0 && m) atomicAdd(totals + 1, (unsigned long long)__popc(m));
 }
 
-struct SceneWave {
-  Ray36 *rays = nullptr, *ao_rays = nullptr;
-  uint32_t *pix = nullptr, *ao_pix = nullptr;
-  SceneHit32 *hits = nullptr;
-  uint8_t *mask = nullptr;
-  unsigned long long *counters = nullptr;  // [0] AO rays of the wave, [1] valid primaries; [4..6] totals
-  void release() {
-    cudaFree(rays), cudaFree(ao_rays), cudaFree(pix), cudaFree(ao_pix), cudaFree(hits), cudaFree(mask), cudaFree(counters);
-  }
-};
-
 }  // namespace
 }  // namespace nrt
 
@@ -970,81 +960,67 @@ extern "C" int nrt_scene_render_ao_device(const nrt_scene *s, const nrt_ao_param
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const uint32_t trav_flags = p.flags & 0xFFFFu;
   // this shard's ray slots: whole tiles, dealt round-robin (render.cu: run_ao_pass)
-  const unsigned long long tiles_x = (p.width + p.tile_w - 1) / p.tile_w, tiles_y = (p.height + p.tile_h - 1) / p.tile_h;
-  const unsigned long long n_tiles = tiles_x * tiles_y;
-  const unsigned long long my_tiles = n_tiles > p.shard ? (n_tiles - p.shard + p.n_shards - 1) / p.n_shards : 0;
-  const unsigned long long per_tile = (unsigned long long)p.tile_w * p.tile_h * p.spp;
-  const unsigned long long slots = my_tiles * per_tile;
-  unsigned long long wave = std::max<unsigned long long>(per_tile, (((unsigned long long)1 << 22) / per_tile) * per_tile);
-  if (wave > slots) wave = slots;
+  const ShardSlots sh = shard_slots(p.width, p.height, p.tile_w, p.tile_h, p.spp, p.shard, p.n_shards);
+  const unsigned long long slots = sh.total, wave = sh.wave(1ull << 22);
   if (wave > 0xFFFFFFF0ull) {
     set_error("nrt_scene_render_ao_device: a tile holds too many ray slots");
     return NRT_ERR_INVALID;
   }
-  SceneWave w;
+  CallMemory mem(st);
+  Ray36 *rays = nullptr, *ao_rays = nullptr;
+  uint32_t *pix = nullptr, *ao_pix = nullptr;
+  SceneHit32 *hits = nullptr;
+  uint8_t *mask = nullptr;
+  unsigned long long *counters = nullptr;  // [0] AO rays of the wave, [1] valid primaries; [4..6] totals
   unsigned long long h_tot[3] = {0, 0, 0};
   uint32_t launches = 0, trav_launches = 0;
-  int rc = NRT_OK;
-  cudaError_t e = cudaSuccess;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+  PassClock clock(res != nullptr);
   if (slots > 0) {
-    e = cudaMalloc(&w.rays, sizeof(Ray36) * wave);
-    if (e == cudaSuccess) e = cudaMalloc(&w.ao_rays, sizeof(Ray36) * wave);
-    if (e == cudaSuccess) e = cudaMalloc(&w.pix, sizeof(uint32_t) * wave);
-    if (e == cudaSuccess) e = cudaMalloc(&w.ao_pix, sizeof(uint32_t) * wave);
-    if (e == cudaSuccess) e = cudaMalloc(&w.hits, sizeof(SceneHit32) * wave);
-    if (e == cudaSuccess) e = cudaMalloc(&w.mask, wave);
-    if (e == cudaSuccess) e = cudaMalloc(&w.counters, sizeof(unsigned long long) * 8);
-    if (e == cudaSuccess) e = cudaMemsetAsync(w.counters, 0, sizeof(unsigned long long) * 8, st);
-    if (e == cudaSuccess) e = cudaEventCreate(&ev0);
-    if (e == cudaSuccess) e = cudaEventCreate(&ev1);
-    if (e == cudaSuccess) e = cudaEventRecord(ev0, st);
+    if (const int rc = mem.alloc([&](Carver &c) {
+          rays = c.take<Ray36>(wave);
+          ao_rays = c.take<Ray36>(wave);
+          pix = c.take<uint32_t>(wave);
+          ao_pix = c.take<uint32_t>(wave);
+          hits = c.take<SceneHit32>(wave);
+          mask = c.take<uint8_t>(wave);
+          counters = c.take<unsigned long long>(8);
+        }))
+      return rc;
+    NRT_CUDA(cudaMemsetAsync(counters, 0, sizeof(unsigned long long) * 8, st));
+    if (const int rc = clock.start(st)) return rc;
   }
-  for (unsigned long long slot0 = 0; slot0 < slots && e == cudaSuccess && rc == NRT_OK; slot0 += wave) {
+  for (unsigned long long slot0 = 0; slot0 < slots; slot0 += wave) {
     const uint32_t count = (uint32_t)std::min(wave, slots - slot0);
     const unsigned blocks = (count + 255) / 256;
-    e = cudaMemsetAsync(w.counters, 0, sizeof(unsigned long long) * 2, st);
-    if (e != cudaSuccess) break;
-    scene_gen_primary_kernel<<<blocks, 256, 0, st>>>(p, slot0, count, w.rays, w.pix, w.counters);
-    rc = scene_launch(sc, w.rays, count, w.hits, w.mask, trav_flags, st);
-    if (rc != NRT_OK) break;
-    scene_gen_ao_kernel<<<blocks, 256, 0, st>>>(p, slot0, count, w.rays, w.pix, w.hits, w.mask, sc->d_inst, w.ao_rays, w.ao_pix,
-                                                d_accum, w.counters);
+    NRT_CUDA(cudaMemsetAsync(counters, 0, sizeof(unsigned long long) * 2, st));
+    scene_gen_primary_kernel<<<blocks, 256, 0, st>>>(p, slot0, count, rays, pix, counters);
+    if (const int rc = scene_launch(sc, rays, count, hits, mask, trav_flags, st)) return rc;
+    scene_gen_ao_kernel<<<blocks, 256, 0, st>>>(p, slot0, count, rays, pix, hits, mask, sc->d_inst, ao_rays, ao_pix,
+                                                d_accum, counters);
     unsigned long long h_cnt[2] = {0, 0};
-    e = cudaMemcpyAsync(h_cnt, w.counters, sizeof(h_cnt), cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);  // the scene walk takes its ray count from the host
-    if (e != cudaSuccess) break;
+    NRT_CUDA(cudaMemcpyAsync(h_cnt, counters, sizeof(h_cnt), cudaMemcpyDeviceToHost, st));
+    NRT_CUDA(cudaStreamSynchronize(st));  // the scene walk takes its ray count from the host
     launches += 3;
     trav_launches += 1;
     h_tot[0] += h_cnt[0];
     h_tot[2] += h_cnt[1];
     if (h_cnt[0] > 0) {
-      rc = scene_launch(sc, w.ao_rays, (size_t)h_cnt[0], w.hits, w.mask, trav_flags, st);
-      if (rc != NRT_OK) break;
-      scene_accumulate_ao_kernel<<<(unsigned)((h_cnt[0] + 255) / 256), 256, 0, st>>>(w.mask, w.hits, w.ao_pix, h_cnt[0], p.ao_max_t,
-                                                                                       d_accum, w.counters + 4);
+      if (const int rc = scene_launch(sc, ao_rays, (size_t)h_cnt[0], hits, mask, trav_flags, st)) return rc;
+      scene_accumulate_ao_kernel<<<(unsigned)((h_cnt[0] + 255) / 256), 256, 0, st>>>(mask, hits, ao_pix, h_cnt[0],
+                                                                                       p.ao_max_t, d_accum, counters + 4);
       launches += 2;
       trav_launches += 1;
     }
-    e = cudaGetLastError();
+    NRT_CUDA(cudaGetLastError());
   }
-  float total_ms = 0.0f;
-  if (slots > 0 && e == cudaSuccess && rc == NRT_OK) {
-    e = cudaEventRecord(ev1, st);
-    unsigned long long h_occ = 0;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&h_occ, w.counters + 5, sizeof(h_occ), cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e == cudaSuccess) e = cudaEventElapsedTime(&total_ms, ev0, ev1);
-    h_tot[1] = h_occ;
-  } else if (slots > 0) {
-    cudaStreamSynchronize(st);  // nothing of a failed pass may still be running on the buffers freed below
+  if (slots > 0) {
+    if (const int rc = clock.stop(st)) return rc;
+    NRT_CUDA(cudaMemcpyAsync(&h_tot[1], counters + 5, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    NRT_CUDA(cudaStreamSynchronize(st));
   }
-  if (ev0) cudaEventDestroy(ev0);
-  if (ev1) cudaEventDestroy(ev1);
-  w.release();
-  if (rc != NRT_OK) return rc;
-  NRT_CUDA(e);
   if (res) {
+    float total_ms = 0.0f, span[2];
+    if (const int rc = clock.read(&total_ms, span)) return rc;
     res->primary_rays = h_tot[2];
     res->ao_rays = h_tot[0];
     res->ao_hits = h_tot[1];
@@ -1054,7 +1030,7 @@ extern "C" int nrt_scene_render_ao_device(const nrt_scene *s, const nrt_ao_param
     res->launches = launches;
     res->traverse_launches = trav_launches;
   }
-  return NRT_OK;
+  return mem.drain();
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -1175,18 +1151,15 @@ __global__ void __launch_bounds__(256)
 }  // namespace
 
 int scene_path_setup(const char *name, const nrt_scene *s, const nrt_path_params &p, const nrt_scene_shading *shading,
-                     size_t cap, cudaStream_t st, ScenePathCall &c) {
-  auto refuse = [&](const char *why) {
-    set_error(std::string(name) + ": " + why);
-    return NRT_ERR_INVALID;
-  };
-  if (!shading) return refuse("NULL shading array (one nrt_scene_shading per instance)");
+                     size_t cap, cudaStream_t st, CallMemory &mem, ScenePathCall &c) {
+  if (!shading) return refuse(name, "NULL shading array (one nrt_scene_shading per instance)");
   if (p.d_material_ids || p.d_facevarying_normals)
-    return refuse("material ids and face-varying normals are given per instance (nrt_scene_shading), not in the params");
-  if (p.flags & NRT_TRAVERSE_ANY_HIT) return refuse("NRT_TRAVERSE_ANY_HIT is not supported by the scene walk");
+    return refuse(name,
+                  "material ids and face-varying normals are given per instance (nrt_scene_shading), not in the params");
+  if (p.flags & NRT_TRAVERSE_ANY_HIT) return refuse(name, "NRT_TRAVERSE_ANY_HIT is not supported by the scene walk");
   Scene *sc = const_cast<Scene *>(reinterpret_cast<const Scene *>(s));
   for (uint32_t i = 0; i < sc->n; i++)
-    if (sc->n_faces[i] == 0) return refuse("triangle instances only");
+    if (sc->n_faces[i] == 0) return refuse(name, "triangle instances only");
   c.s = s;
   c.p = p;
   c.trav_flags = p.flags & 0xFFFFu;
@@ -1197,24 +1170,26 @@ int scene_path_setup(const char *name, const nrt_scene *s, const nrt_path_params
     NRT_CUDA(cudaStreamSynchronize(st));
     for (uint32_t k = 0; k < p.n_emissive; k++)
       if (pairs[2 * k] >= sc->n || pairs[2 * k + 1] >= sc->n_faces[pairs[2 * k]])
-        return refuse(("emissive pair " + std::to_string(k) + " is not an {instance, face} of the scene").c_str());
+        return refuse(name, ("emissive pair " + std::to_string(k) + " is not an {instance, face} of the scene").c_str());
   }
-  NRT_CUDA(cudaMalloc(&c.shading, sizeof(SceneShadingDev) * sc->n));
-  NRT_CUDA(cudaMalloc(&c.ctr, sizeof(unsigned long long) * 4));
+  const bool lights = p.n_emissive && cap > 0;
+  if (const int rc = mem.alloc([&](Carver &k) {
+        c.shading = k.take<SceneShadingDev>(sc->n);
+        c.ctr = k.take<unsigned long long>(4);
+        if (lights) c.lights = k.take<float4>(4 * (size_t)p.n_emissive);
+        c.rays = k.take<Ray36>(cap);
+        c.hits = k.take<SceneHit32>(cap);
+        c.mask = k.take<uint8_t>(cap);
+      }))
+    return rc;
   NRT_CUDA(cudaMemcpyAsync(c.shading, shading, sizeof(SceneShadingDev) * sc->n, cudaMemcpyHostToDevice, st));
-  if (p.n_emissive && cap > 0) {
-    NRT_CUDA(cudaMalloc(&c.lights, 4 * sizeof(float4) * p.n_emissive));
+  if (lights) {
     scene_light_setup_kernel<<<(p.n_emissive + 127) / 128, 128, 0, st>>>(
         static_cast<const uint32_t *>(p.d_emissive_faces), p.n_emissive, sc->d_inst,
         c.shading, static_cast<const PathMaterial *>(p.d_materials),
         c.lights);
     NRT_CUDA(cudaGetLastError());
     c.launches++;
-  }
-  if (cap > 0) {
-    NRT_CUDA(cudaMalloc(&c.rays, sizeof(Ray36) * cap));
-    NRT_CUDA(cudaMalloc(&c.hits, sizeof(SceneHit32) * cap));
-    NRT_CUDA(cudaMalloc(&c.mask, cap));
   }
   return NRT_OK;
 }
@@ -1236,21 +1211,11 @@ int scene_shadow_pass(ScenePathCall &c, const PathQueues &q, uint32_t ns, float 
 
 namespace {
 
-// Checks the path pass's own parameters (nothing is launched when they are refused), then scene_path_setup.
-int scene_path_begin(const char *name, const nrt_scene *s, const nrt_path_params *pp, const nrt_scene_shading *shading,
-                     size_t cap, cudaStream_t st, ScenePathCall &c) {
-  auto refuse = [&](const char *why) {
-    set_error(std::string(name) + ": " + why);
-    return NRT_ERR_INVALID;
-  };
-  if (!s || !pp) return refuse("NULL argument");
-  const nrt_path_params p = *pp;
-  if (p.width == 0 || p.height == 0 || p.spp == 0 || p.n_shards == 0 || p.shard >= p.n_shards || p.tile_w == 0 ||
-      p.tile_h == 0 || (p.tile_w % 8) != 0 || (p.tile_h % 4) != 0 || p.max_bounces == 0 || p.n_materials == 0 ||
-      !p.d_materials || (p.n_emissive > 0 && !p.d_emissive_faces))
-    return refuse("bad parameters");
-  if (p.flags & NRT_AO_PACKED_TILES) return refuse("NRT_AO_PACKED_TILES is not supported");
-  return scene_path_setup(name, s, p, shading, cap, st, c);
+// The path pass's own rules on its parameters, before scene_path_setup's (nothing is launched when they are refused)
+int scene_path_check(const char *name, const nrt_path_params &p) {
+  if (const int rc = check_path_params(p, name)) return rc;
+  if (p.flags & NRT_AO_PACKED_TILES) return refuse(name, "NRT_AO_PACKED_TILES is not supported");
+  return NRT_OK;
 }
 
 // One bounce: walk the n rays of queue `in`, shade them (Slots: TileSlots or TexelSlots), read the counts;
@@ -1294,93 +1259,48 @@ int scene_texel_bounce(ScenePathCall &c, const TexelSlots &slots, uint32_t bounc
 extern "C" int nrt_scene_render_path_device(const nrt_scene *s, const nrt_path_params *pp,
                                             const nrt_scene_shading *shading, float *d_accum_rgb, nrt_path_result *res,
                                             void *stream) {
-  if (!s || !pp || !d_accum_rgb) {
-    set_error("nrt_scene_render_path_device: NULL argument");
-    return NRT_ERR_INVALID;
-  }
+  static const char *who = "nrt_scene_render_path_device";
+  if (!s || !pp || !d_accum_rgb) return refuse(who, "NULL argument");
+  const nrt_path_params p = *pp;
+  if (const int rc = scene_path_check(who, p)) return rc;
   const Scene *sc = reinterpret_cast<const Scene *>(s);
   NRT_DEVICE(sc->device);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const nrt_path_params p = *pp;
   // this shard's ray slots: whole tiles, dealt round-robin, in waves of whole tiles (nrt_scene_render_ao_device)
-  const unsigned long long tiles_x = p.tile_w ? (p.width + p.tile_w - 1) / p.tile_w : 0;
-  const unsigned long long tiles_y = p.tile_h ? (p.height + p.tile_h - 1) / p.tile_h : 0;
-  const unsigned long long n_tiles = tiles_x * tiles_y;
-  const unsigned long long my_tiles =
-      (p.n_shards && n_tiles > p.shard) ? (n_tiles - p.shard + p.n_shards - 1) / p.n_shards : 0;
-  const unsigned long long per_tile = (unsigned long long)p.tile_w * p.tile_h * p.spp;
-  const unsigned long long slots = my_tiles * per_tile;
-  unsigned long long wave =
-      per_tile ? std::max<unsigned long long>(per_tile, (((unsigned long long)1 << 22) / per_tile) * per_tile) : 0;
-  if (wave > slots) wave = slots;
-  if (wave > 0xFFFFFFF0ull) {
-    set_error("nrt_scene_render_path_device: a tile holds too many ray slots");
-    return NRT_ERR_INVALID;
-  }
+  const ShardSlots sh = shard_slots(p.width, p.height, p.tile_w, p.tile_h, p.spp, p.shard, p.n_shards);
+  const unsigned long long slots = sh.total, wave = sh.wave(1ull << 22);
+  if (wave > 0xFFFFFFF0ull) return refuse(who, "a tile holds too many ray slots");
+  CallMemory mem(st);
   ScenePathCall c;
-  int rc = scene_path_begin("nrt_scene_render_path_device", s, pp, shading, (size_t)wave, st, c);
-  if (rc != NRT_OK) {
-    cudaStreamSynchronize(st);  // nothing of a failed set-up may still use the buffers freed on return
-    return rc;
-  }
-  // per path: 2 radiance queues, the shadow queue, the throughput
+  if (const int rc = scene_path_setup(who, s, p, shading, (size_t)wave, st, mem, c)) return rc;
   PathQueues q;
-  std::vector<void *> bufs;
-  cudaError_t e = cudaSuccess;
-  auto alloc = [&](size_t bytes) -> void * {
-    void *ptr = nullptr;
-    if (e == cudaSuccess) e = cudaMalloc(&ptr, bytes ? bytes : 1);
-    bufs.push_back(ptr);
-    return ptr;
-  };
-  for (int k = 0; k < 2; k++) {
-    q.org_tmin[k] = static_cast<float4 *>(alloc(sizeof(float4) * wave));
-    q.dir_tmax[k] = static_cast<float4 *>(alloc(sizeof(float4) * wave));
-    q.path_id[k] = static_cast<uint32_t *>(alloc(sizeof(uint32_t) * wave));
-  }
-  q.sh_org_tmin = static_cast<float4 *>(alloc(sizeof(float4) * wave));
-  q.sh_dir_tmax = static_cast<float4 *>(alloc(sizeof(float4) * wave));
-  q.sh_contrib_pix = static_cast<float4 *>(alloc(sizeof(float4) * wave));
-  q.weight = static_cast<float4 *>(alloc(sizeof(float4) * wave));
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  if (e == cudaSuccess) e = cudaEventCreate(&ev0);
-  if (e == cudaSuccess) e = cudaEventCreate(&ev1);
-  if (e == cudaSuccess) e = cudaEventRecord(ev0, st);
+  if (const int rc = mem.alloc([&](Carver &k) { q = carve_path_queues(k, wave); })) return rc;
+  PassClock clock(res != nullptr);
+  if (const int rc = clock.start(st)) return rc;
   unsigned long long camera = 0, radiance = 0, shadow = 0;
-  for (unsigned long long slot0 = 0; slot0 < slots && e == cudaSuccess && rc == NRT_OK; slot0 += wave) {
+  for (unsigned long long slot0 = 0; slot0 < slots; slot0 += wave) {
     const uint32_t count = (uint32_t)std::min(wave, slots - slot0);
-    e = cudaMemsetAsync(c.ctr, 0, 4 * sizeof(unsigned long long), st);
-    if (e != cudaSuccess) break;
+    NRT_CUDA(cudaMemsetAsync(c.ctr, 0, 4 * sizeof(unsigned long long), st));
     launch_path_camera(p, slot0, count, q, c.ctr, st);
     c.launches++;
     uint32_t n = count;
     int in = 0;
     for (uint32_t b = 0; b < p.max_bounces && n > 0; b++) {
       unsigned long long out[3];
-      rc = scene_path_bounce(c, slot0, b, n, q, in, d_accum_rgb, true, out, st);
-      if (rc != NRT_OK) break;
+      if (const int rc = scene_path_bounce(c, slot0, b, n, q, in, d_accum_rgb, true, out, st)) return rc;
       if (b == 0) camera += out[2];
       radiance += b == 0 ? out[2] : n;  // slots outside the image are no Traverse calls
       shadow += out[1];
       n = (uint32_t)out[0];
       in ^= 1;
     }
-    if (e == cudaSuccess) e = cudaGetLastError();
+    NRT_CUDA(cudaGetLastError());
   }
-  float total_ms = 0.0f;
-  if (e == cudaSuccess && rc == NRT_OK) {
-    e = cudaEventRecord(ev1, st);
-    if (e == cudaSuccess) e = cudaEventSynchronize(ev1);
-    if (e == cudaSuccess) e = cudaEventElapsedTime(&total_ms, ev0, ev1);
-  } else {
-    cudaStreamSynchronize(st);  // nothing of a failed pass may still be running on the buffers freed below
-  }
-  if (ev0) cudaEventDestroy(ev0);
-  if (ev1) cudaEventDestroy(ev1);
-  for (void *ptr : bufs) cudaFree(ptr);
-  if (rc != NRT_OK) return rc;
-  NRT_CUDA(e);
+  if (const int rc = clock.stop(st)) return rc;
+  if (const int rc = mem.drain()) return rc;
   if (res) {
+    float total_ms = 0.0f, span[2];
+    if (const int rc = clock.read(&total_ms, span)) return rc;
     res->camera_rays = camera;
     res->radiance_rays = radiance;
     res->shadow_rays = shadow;
@@ -1399,43 +1319,26 @@ extern "C" int nrt_scene_path_bounce_device(const nrt_scene *s, const nrt_path_p
                                             uint32_t *d_out_path_id, void *d_sh_org_tmin, void *d_sh_dir_tmax,
                                             void *d_sh_contrib_pix, float *d_accum_rgb, uint64_t *n_continue,
                                             uint64_t *n_shadow, int skip_shadow_pass, void *stream) {
+  static const char *who = "nrt_scene_path_bounce_device";
   if (!s || !pp || !d_org_tmin || !d_dir_tmax || !d_path_id || !d_weight || !d_out_org_tmin || !d_out_dir_tmax ||
-      !d_out_path_id || !d_sh_org_tmin || !d_sh_dir_tmax || !d_sh_contrib_pix || !d_accum_rgb) {
-    set_error("nrt_scene_path_bounce_device: NULL argument");
-    return NRT_ERR_INVALID;
-  }
+      !d_out_path_id || !d_sh_org_tmin || !d_sh_dir_tmax || !d_sh_contrib_pix || !d_accum_rgb)
+    return refuse(who, "NULL argument");
   if (n_continue) *n_continue = 0;
   if (n_shadow) *n_shadow = 0;
-  if (n_rays > 0xFFFFFFF0ull) {
-    set_error("nrt_scene_path_bounce_device: more than 2^32 - 16 rays");
-    return NRT_ERR_INVALID;
-  }
+  if (n_rays > 0xFFFFFFF0ull) return refuse(who, "more than 2^32 - 16 rays");
+  const nrt_path_params p = *pp;
+  if (const int rc = scene_path_check(who, p)) return rc;
   const Scene *sc = reinterpret_cast<const Scene *>(s);
   NRT_DEVICE(sc->device);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CallMemory mem(st);
   ScenePathCall c;
-  int rc = scene_path_begin("nrt_scene_path_bounce_device", s, pp, shading, (size_t)n_rays, st, c);
-  if (rc == NRT_OK && n_rays > 0) {
-    PathQueues q;
-    q.org_tmin[0] = static_cast<float4 *>(const_cast<void *>(d_org_tmin));
-    q.dir_tmax[0] = static_cast<float4 *>(const_cast<void *>(d_dir_tmax));
-    q.path_id[0] = const_cast<uint32_t *>(d_path_id);
-    q.org_tmin[1] = static_cast<float4 *>(d_out_org_tmin);
-    q.dir_tmax[1] = static_cast<float4 *>(d_out_dir_tmax);
-    q.path_id[1] = d_out_path_id;
-    q.sh_org_tmin = static_cast<float4 *>(d_sh_org_tmin);
-    q.sh_dir_tmax = static_cast<float4 *>(d_sh_dir_tmax);
-    q.sh_contrib_pix = static_cast<float4 *>(d_sh_contrib_pix);
-    q.weight = static_cast<float4 *>(d_weight);
-    unsigned long long out[3] = {0, 0, 0};
-    rc = scene_path_bounce(c, 0ull, bounce, (uint32_t)n_rays, q, 0, d_accum_rgb, !skip_shadow_pass, out, st);
-    if (rc == NRT_OK) {
-      if (n_continue) *n_continue = out[0];
-      if (n_shadow) *n_shadow = out[1];
-    }
-  }
-  const cudaError_t e = cudaStreamSynchronize(st);  // the call's buffers are freed on return
-  if (rc != NRT_OK) return rc;
-  NRT_CUDA(e);
-  return NRT_OK;
+  if (const int rc = scene_path_setup(who, s, p, shading, (size_t)n_rays, st, mem, c)) return rc;
+  if (n_rays == 0) return mem.drain();
+  const PathQueues q = caller_path_queues(d_org_tmin, d_dir_tmax, d_path_id, d_weight, d_out_org_tmin, d_out_dir_tmax,
+                                         d_out_path_id, d_sh_org_tmin, d_sh_dir_tmax, d_sh_contrib_pix);
+  unsigned long long out[3] = {0, 0, 0};
+  if (const int rc = scene_path_bounce(c, 0ull, bounce, (uint32_t)n_rays, q, 0, d_accum_rgb, !skip_shadow_pass, out, st))
+    return rc;
+  return finish_bounce(nullptr, out, n_continue, n_shadow, st);
 }

@@ -181,8 +181,10 @@ SceneView scene_view(const nrt_scene *s);
 int scene_walk(const nrt_scene *s, const Ray36 *d_rays, size_t n, void *d_hits, uint8_t *d_mask, uint32_t flags,
                cudaStream_t st);
 
-// What one scene path or lightmap call owns on the device: the per-instance shading table, the world-space light
-// records (SceneLights) and the walk's buffers.
+class CallMemory;  // pass_host.cuh
+
+// What one scene path or lightmap call keeps on the device, in its CallMemory: the per-instance shading table, the
+// world-space light records (SceneLights) and the walk's buffers.
 struct ScenePathCall {
   const nrt_scene *s = nullptr;
   nrt_path_params p{};
@@ -194,15 +196,12 @@ struct ScenePathCall {
   uint8_t *mask = nullptr;
   unsigned long long *ctr = nullptr;  // [0] continuation rays, [1] shadow rays, [2] camera rays
   uint32_t launches = 0, trav_launches = 0;
-  ~ScenePathCall() {
-    cudaFree(shading), cudaFree(lights), cudaFree(rays), cudaFree(hits), cudaFree(mask), cudaFree(ctr);
-  }
 };
 // The set-up both scene.cu's path pass and the scene lightmap bake start with, after their own parameter checks:
 // refuses a NULL shading array, material ids or normals in p, ANY_HIT, a non-triangle instance and an emissive pair
-// that is no {instance, face} of the scene (read back once); then allocates the call's buffers for `cap` rays and
-// writes the shading table and the light records.
+// that is no {instance, face} of the scene (read back once); then allocates the call's buffers for `cap` rays in mem
+// and writes the shading table and the light records.
 int scene_path_setup(const char *name, const nrt_scene *s, const nrt_path_params &p, const nrt_scene_shading *shading,
-                     size_t cap, cudaStream_t st, ScenePathCall &c);
+                     size_t cap, cudaStream_t st, CallMemory &mem, ScenePathCall &c);
 
 }  // namespace nrt

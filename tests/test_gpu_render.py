@@ -149,3 +149,26 @@ def test_any_hit_occlusion_rays_give_the_same_frame(name, kw, W, H, spp):
         o = api.BVHTraceOptions(prim_ids_range=(int(ah["prim_id"][i]), int(ah["prim_id"][i]) + 1))
         h1, m1 = acc.Traverse(ao[i:i + 1], options=o)
         assert m1[0] == 1 and h1.view(np.uint32).tolist() == ah[i:i + 1].view(np.uint32).tolist()
+
+
+@pytest.mark.parametrize("unfused", [False, True])
+def test_pass_times_split_into_primary_and_ao_launches(unfused):
+    """The AO pass's traversal time is the sum of its camera-ray and AO-ray launch times, both inside the pass's time;
+    with no result struct the pass renders the same frame."""
+    import torch
+    from nanort_b200 import api, scenes as S
+
+    name, W, H, spp = "sphere_grid", 200, 104, 2
+    v, f = S.make_scene(name, nx=4, nz=4)
+    acc = api.BVHAccel()
+    acc.Build(len(f), v, f)
+    p, _ = _params(api, S, name, W, H, spp, acc.BoundingBox(), flags=api.AO_UNFUSED if unfused else 0)
+    accum = torch.zeros(W * H, dtype=torch.float32, device="cuda")
+    r = acc.RenderAO(p, accum.data_ptr())
+    assert r.primary_traverse_ms > 0.0 and r.ao_traverse_ms > 0.0
+    assert abs(r.traverse_ms - (r.primary_traverse_ms + r.ao_traverse_ms)) <= 1e-4 * r.traverse_ms
+    assert r.traverse_ms <= r.total_ms
+    quiet = torch.zeros(W * H, dtype=torch.float32, device="cuda")
+    acc.RenderAO(p, quiet.data_ptr(), want_result=False)
+    torch.cuda.synchronize()
+    assert torch.equal(quiet, accum)

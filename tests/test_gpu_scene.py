@@ -222,3 +222,26 @@ def test_scene_ao_pass_against_the_flattened_scene():
         total += part
         rays += r.primary_rays
     assert rays == W * H * spp and torch.equal(total, a_sc)
+
+
+def test_scene_ao_pass_without_a_result():
+    """nrt_scene_render_ao_device with res == NULL, which the C ABI allows: the call succeeds and renders the frame it
+    renders with a result struct, bit for bit (nothing is timed)."""
+    import ctypes as C
+
+    import torch
+    from nanort_b200 import api, scenes as S
+
+    base = S.sphere_grid(nx=2, nz=2)
+    insts = [(base[0], base[1], S.xform(translate=(-4.0, 0.0, 0.0))),
+             (base[0], base[1], S.xform(translate=(4.0, 0.5, 1.0), yaw=0.6))]
+    sc = _gpu_scene(insts, api.BUILD_FAST, api.BUILD_FAST)
+    W, H, spp = 160, 96, 2
+    p = _ao_params(api, S.look_at((0.0, 8.0, 18.0), (0.0, 0.0, 0.0), aspect=W / H), W, H, spp, 3.0)
+    with_res = torch.zeros(W * H, dtype=torch.float32, device="cuda")
+    r = sc.RenderAO(p, with_res.data_ptr())
+    assert r.primary_rays == W * H * spp and r.ao_hits > 0
+    without = torch.zeros(W * H, dtype=torch.float32, device="cuda")
+    rc = api.lib().nrt_scene_render_ao_device(sc._h, C.byref(p), C.c_void_p(without.data_ptr()), None, None)
+    assert rc == 0, api.lib().nrt_last_error()
+    assert torch.equal(without, with_res)
